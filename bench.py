@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py -- Marlin prover throughput on B200 (BASELINE.json metric: prover constraints/sec, BLS12-381).
+"""bench.py -- Marlin prover throughput on H100 (BASELINE.json metric: prover constraints/sec, BLS12-381).
 
 A "step" is one `Marlin::prove` (reference src/lib.rs:151-311) of the reference bench's DummyCircuit
 (benches/bench.rs:25-67) scaled to 2^log_n constraints; SRS generation and `index` are outside the
@@ -9,7 +9,7 @@ timed region exactly as in benches/bench.rs:79-101.
   e2e   : the same through the public API with HOST buffers -- host->device copy of the instance and
           device->host read of the proof inside the timed region
   roofline     : the dominant kernel (msm_accumulate_kernel) -- algorithmic bytes (128 B per
-                 (base, scalar) pair, SURVEY.md section 8d) / CUDA-event kernel time / measured HBM peak
+                 (base, scalar) pair, SURVEY.md section 8d) / CUDA-event kernel time / HBM peak
   cpu_baseline : the oracle's C++ restatement of the reference prover (oracle/cport/prover.cpp) timed on this
                  box's host cores (rank 0, N = 1) on a bounded sample: full proves of a 2^16-constraint
                  instance of the same circuit family (~10-30 s of CPU work)
@@ -18,8 +18,13 @@ timed region exactly as in benches/bench.rs:79-101.
 N > 1 (torchrun, one rank per GPU): every rank runs the prover, each MSM is sharded by base/scalar
 chunk and the partial sums are exchanged with one NCCL all-gather per MSM (DESIGN.md "Multi-GPU");
 total work is fixed => "scaling": "strong".
+
+--dump-outputs DIR writes what the last timed step returned to its caller -- the proof bytes of the device-resident
+prove (proof.npy) and of the host-buffer prove (proof_e2e.npy), one float32 per byte -- so that two builds can be compared
+output for output; every input (circuit, SRS trapdoor, zk stream) is fixed, so the same arguments give the same inputs.
 """
 import argparse
+import atexit
 import json
 import os
 import subprocess
@@ -34,7 +39,7 @@ sys.path.insert(0, ROOT)
 def parse_args():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--steps", type=int, default=5, help="timed proves per timed region (at least 1)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--log-n", type=int, default=20, help="log2 of the number of constraints (BASELINE config 2: 20)")
@@ -49,7 +54,11 @@ def parse_args():
     ap.add_argument("--no-verify", action="store_true", help="skip the post-run proof check (oracle verifier with the real pairing)")
     ap.add_argument("--save-proof", default=None, help="write the hashed proof, the verifier key and the public data to this JSON file "
                                                        "(checked afterwards on a CPU by tests/verify_saved_proof.py)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the proofs of the last timed steps to DIR/*.npy")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    return args
 
 
 def measured_peaks():
@@ -57,11 +66,11 @@ def measured_peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return json.load(f), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0}, "fallback"
+        return {"hbm_gbs": 3350.0}, "datasheet (H100 SXM, 700 W)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md): one
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region: one
     long-running `nvidia-smi -lms` process started before the warm-up (so its start-up cost never lands
     in a timed step); mark() brackets the timed region and only samples inside it are summarised."""
     FIELDS = ("timestamp,clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -76,6 +85,7 @@ class ClockSampler:
                                           "-lms", str(period_ms)], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
             self.t = threading.Thread(target=self._pump, daemon=True)
             self.t.start()
+            atexit.register(self.close)  # never leave the sampler running, also when the bench fails
         except Exception:
             self.proc = None
         self.t0 = self.t1 = None
@@ -206,7 +216,7 @@ def main():
     clocks.begin()
     t0 = time.perf_counter()
     for _ in range(args.steps):
-        m.prove(pk, None, zk)
+        proof_dev = m.prove(pk, None, zk)
         dev_ms.append(pk.timings()["Marlin::Prover"])  # CUDA events on the library's stream
     barrier()
     wall = time.perf_counter() - t0
@@ -229,6 +239,11 @@ def main():
     barrier()
     wall_e2e = time.perf_counter() - t0
     clocks.close()
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, blob in (("proof", proof_dev), ("proof_e2e", proof)):
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), np.frombuffer(blob, dtype=np.uint8).astype(np.float32))
     # outside every timed region: a proof from a fresh zk stream, hashed, so that runs with different window sizes,
     # GPU counts or library builds can be compared byte for byte
     import hashlib
@@ -286,7 +301,7 @@ def main():
     scalar_bits = 255 if args.curve == "bls12_381" else 254
     msm_windows, mul_peak = (scalar_bits + win_bits) // win_bits, None  # signed c-bit windows per scalar (c = 20 -> 13)
     try:
-        with open(os.path.join(ROOT, "profiles", "r02_microbench_int_alu.json")) as f:
+        with open(os.path.join(ROOT, "profiles", "h100_microbench_int_alu.json")) as f:
             mb = json.load(f)
         mul_peak = max(v for k, v in mb.items() if k.startswith("fq_mul")) if args.curve == "bls12_381" else None
     except Exception:
@@ -295,15 +310,6 @@ def main():
     # addition 10; L levels leave 1/2^L of the references to the XYZZ kernel
     share = 0.5 ** aff_levels
     muls = msm_windows * (lev["units"] * ((1 - share) * 6 + share * 10) + (acc["units"] - lev["units"]) * 10)
-    traffic = None  # DRAM bytes per launch from the committed `ncu --set full` capture of THIS round's kernels (profiles/), scaled to this run's mean launch
-    try:
-        with open(os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")) as f:
-            tr = json.load(f)
-        if args.curve == "bls12_381" and acc["launches"]:
-            per_pair = (tr["levels"]["dram_bytes_per_pair"] + tr["accumulate_after_levels"]["dram_bytes_per_pair"]) if lev["launches"] else tr["dram_bytes_per_pair"]
-            traffic = per_pair * acc["units"] / acc["launches"]
-    except Exception:
-        pass
     line = {
         "metric": "prover_constraints_per_sec", "value": value, "unit": "constraints/s", "n_gpus": world, "steps": args.steps,
         "warmup": max(args.warmup, 3), "ms_per_step": ms_step, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
@@ -320,19 +326,18 @@ def main():
         "clocks": clocks.summary(),
         "roofline": {"bound": "hbm", "kernel": ("MSM bucket pass: %d batched-affine level kernels (fused level 0, split levels >= 1) + msm_accumulate_kernel" % aff_levels) if lev["launches"]
                      else "msm_accumulate_kernel", "achieved": achieved, "peak": peaks.get("hbm_gbs"), "unit": "GB/s",
-                     "frac": (achieved / peaks["hbm_gbs"]) if achieved else None, "traffic": traffic, "peak_source": peak_kind,
+                     "frac": (achieved / peaks["hbm_gbs"]) if achieved else None, "peak_source": peak_kind,
                      "algorithmic_bytes_per_launch": (acc["units"] * pair_bytes / acc["launches"]) if acc["launches"] else None,
                      "algorithmic_bytes_per_pair": pair_bytes, "launch": "the bucket pass of one MSM (mean over the proof's MSMs)",
-                     "note": "bound by the 32-bit integer multiplier, not by HBM (roofline_int_alu; DESIGN.md Rooflines); traffic = "
-                             "level + accumulate kernels of one 2^22-pair MSM (profiles/r02_ncu_level_accumulate.md)"},
+                     "note": "bound by the 32-bit integer multiplier, not by HBM (roofline_int_alu; DESIGN.md Rooflines)"},
         # the meaningful roofline of these kernels: Fq multiplications per second against the whole-chip
-        # integer-multiply microbenchmark (profiles/r02_microbench_int_alu.json, tools/microbench.cu)
+        # integer-multiply microbenchmark (profiles/h100_microbench_int_alu.json, tools/microbench.cu)
         "roofline_int_alu": {"kernel": "MSM bucket pass", "unit": "G Fq multiplications/s",
                              "achieved": (muls / (bucket_ms / 1e3) / 1e9) if bucket_ms else None,
                              "peak": mul_peak, "frac": (muls / (bucket_ms / 1e3) / 1e9 / mul_peak) if bucket_ms and mul_peak else None,
                              "affine_levels": aff_levels, "muls_per_affine_add": 6, "muls_per_xyzz_add": 10,
                              "bucket_additions_per_s_G": (acc["units"] * msm_windows / (bucket_ms / 1e3) / 1e9) if bucket_ms else None,
-                             "peak_source": "tools/microbench.cu fq_mul (measured on this pool's B200)"},
+                             "peak_source": "tools/microbench.cu fq_mul (profiles/h100_microbench_int_alu.json)"},
         "msm_bucket_pass_ms_per_step": bucket_ms / args.steps if bucket_ms else None,
         "kernels": kern, "phases_ms": phases, "dev_ms_steps": dev_ms, "setup_s": setup_s, "proof_bytes": len(proof), "proof_sha256": proof_sha,
         "proof_verified": proof_verified, "proof_matches_pinned_1gpu_hash": proof_matches, "proof_check": proof_check,

@@ -1,4 +1,4 @@
-/* b2m.h -- C ABI of the B200-native Marlin prover hot path.
+/* b2m.h -- C ABI of the H100-native (sm_90a) Marlin prover hot path.
  *
  * The reference (arkworks-rs/marlin) has no FFI; its seam is the generic parameter
  * `PC: PolynomialCommitment<F, DensePolynomial<F>>` of `Marlin<F, PC, FS>`

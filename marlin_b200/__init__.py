@@ -1,4 +1,4 @@
-"""marlin_b200 -- B200-native (sm_100a) Marlin prover hot path.
+"""marlin_b200 -- H100-native (sm_90a) Marlin prover hot path.
 
 Host-side mirror of the reference's public API for this path
 (`Marlin::<F, PC, FS>::{index, prove}` [reference src/lib.rs:100-311]) over the C ABI in

@@ -15,7 +15,7 @@ using namespace b2m;
 extern "C" {
 
 const char* b2m_last_error(void) { return g_last_error.c_str(); }
-const char* b2m_version(void) { return "b2m 0.1 (sm_100a)"; }
+const char* b2m_version(void) { return "b2m 0.1 (sm_90a)"; }
 
 int b2m_ctx_create(int device, b2m_ctx** out) {
   return guard([&] {

@@ -44,7 +44,7 @@ inline std::string fmt(const char* f, ...) {
 
 struct Ctx {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   cudaStream_t stream = nullptr;  // the stream every helper launches on (see StreamSwap)
   cudaStream_t side = nullptr;    // second stream: sort of the next MSM while the current one accumulates
   cudaMemPool_t pool = nullptr;
@@ -101,7 +101,8 @@ struct Ctx {
     B2M_CUDA(cudaSetDevice(dev));
     cudaDeviceProp prop;
     B2M_CUDA(cudaGetDeviceProperties(&prop, dev));
-    B2M_REQUIRE(prop.major >= 10, B2M_ERR_CUDA, "device %d is sm_%d%d; this library is built for sm_100a only",
+    // the library holds sm_90a SASS and no PTX: it loads on compute capability 9.0 only
+    B2M_REQUIRE(prop.major == 9 && prop.minor == 0, B2M_ERR_CUDA, "device %d is sm_%d%d; this library is built for sm_90a only",
                 dev, prop.major, prop.minor);
     sm_count = prop.multiProcessorCount;
     B2M_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));

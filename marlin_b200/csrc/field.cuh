@@ -1,4 +1,4 @@
-// Montgomery prime-field arithmetic for sm_100a, 32-bit limbs, PTX carry chains.
+// Montgomery prime-field arithmetic for sm_90a, 32-bit limbs, PTX carry chains.
 //
 // Replaces (for the prover hot path) ark-ff 0.3 `Fp256<P>` / `Fp384<P>`
 // [U ark-ff src/fields/models/fp_256.rs, fp_384.rs]: same Montgomery radix

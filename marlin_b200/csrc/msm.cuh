@@ -1,4 +1,4 @@
-// Variable-base multi-scalar multiplication over G1 for sm_100a.
+// Variable-base multi-scalar multiplication over G1 for sm_90a.
 //
 // Replaces ark-ec 0.3 `VariableBaseMSM::multi_scalar_mul(&[G::Affine], &[BigInt])`
 // [U ark-ec src/msm/variable_base.rs] behind `KZG10::commit` / `KZG10::open`, i.e. behind every
@@ -6,7 +6,7 @@
 //
 // The reference runs Pippenger with ~17 windows of c = ln(n)+2 bits, one rayon task per
 // window, 2^c-1 Jacobian buckets each, a running-sum reduction per window and c doublings
-// between windows.  The B200 design trades HBM capacity for all of the doublings and all but
+// between windows.  This design trades HBM capacity for all of the doublings and all but
 // one of the bucket sets: the bases are the FIXED powers of the SRS, so at key-load time we
 // store 2^(c*w) * P_i for every window w (W tables, W*96 B per power; 5.2 GB for 2^22 powers
 // at c = 20).  An MSM is then ONE bucket problem: every (scalar, window) signed digit d sends
@@ -32,7 +32,7 @@ constexpr uint32_t MSM_BKT_MASK = (1u << MSM_BKT_BITS) - 1;
 constexpr uint32_t MSM_NO_DIGIT = 0xffffffffu;
 constexpr int MSM_MAX_BATCH = 8;   // MSMs per run_batch call
 constexpr int MSM_MAX_AFFINE_LEVELS = 6;
-constexpr size_t MSM_AFFINE_MIN_REFS = (size_t)1 << 23;  // MSMs with fewer bucket references skip the batched-affine levels (measured: a loss below ~2^22)
+constexpr size_t MSM_AFFINE_MIN_REFS = (size_t)1 << 23;  // MSMs with fewer bucket references skip the batched-affine levels (latency-bound below)
 
 template <class Fr, class Fq>
 struct MsmJob {
@@ -61,11 +61,12 @@ struct Msm {
   int c = 0, W = 0;
   // batched-affine levels run before the XYZZ bucket pass (msm_affine.cuh); override: B2M_MSM_AFFINE_LEVELS.
   // Off for a 254-bit Fq: its multiplications are so cheap that the levels' extra memory traffic costs more
-  // than the saved multiplications (BN254 2^20: 126.6 ms with, 120.6 ms without).
+  // than the saved multiplications.
   int affine_levels = Fq::N > 8 ? 3 : 0;
-  // levels >= 1 (streaming operands): split kernels with the level-wide batch inversion, 32 additions per chain -- measured
-  // 33.0 + 19.0 ms per 2^20 proof against 36.5 + 20.4 for the fused kernel at T = 64 (level 0 is the other way round: 77.7 vs 82.3)
-  int affine_ctas_upper = 21;  // B2M_MSM_AFFINE_CTAS_UPPER
+  // levels >= 1 (streaming operands): split kernels with the level-wide batch inversion, 32 additions per chain, are faster
+  // than the fused kernel at T = 64; level 0 (random gathers) is the other way round.  On H100 the software-pipelined
+  // addition pass at 3 CTAs/SM (22) beats the plain one at 4 (21) on these levels; level 0 stays with the plain fused kernel.
+  int affine_ctas_upper = 22;  // B2M_MSM_AFFINE_CTAS_UPPER
   int affine_ctas = 4;      // level-kernel variant of level 0 (B2M_MSM_AFFINE_CTAS; the list is at the launch site in msm_impl.cuh)
   size_t affine_min_refs = MSM_AFFINE_MIN_REFS;  // B2M_MSM_AFFINE_MIN_REFS
   int affine_map = 1;       // output -> thread mapping of the levels: 1 = warp-interleaved (coalesced), 0 = blocked; B2M_MSM_AFFINE_MAP

@@ -12,8 +12,7 @@
 // the sums.  After a few levels the remaining points (n / 2^levels) go through the XYZZ bucket pass, which balances any
 // bucket-size distribution.
 //
-// Forms of the arithmetic kernel, all byte-identical in their results (profiles/r02_level_kernel_notes.md has the
-// measurements that chose the defaults):
+// Forms of the arithmetic kernel, all byte-identical in their results (selectable at run time, msm_impl.cuh launch site):
 //   * fused (aff_level_thread): both passes and one binary-Euclid inversion (field.cuh inverse_fast) per thread -- the
 //     default for level 0, whose operands are random gathers from the window tables;
 //   * branch-free and software-pipelined (aff_level_thread_sp, PHASE 0);
@@ -358,7 +357,7 @@ B2M_HD void aff_store_out(const AffLevel<Fq>& A, uint32_t o, const Affine<Fq>& R
 }
 
 // ---- software-pipelined variant (kernel variants 8 / 9) ---------------------------------------------------------------
-// What the captures of the variants above say (profiles/r02_level_kernel_notes.md): no pipe is saturated -- every warp simply
+// Profiles of the variants above show no saturated pipe -- every warp simply
 // runs at its own latency-bound pace (a serial chain of five multiplications per output, each multiplication two carry
 // chains, operand loads issued at their point of use), and extra work of ANY kind (more inversions, more loads) adds its full
 // time.  This variant restructures the per-thread code instead of relying on co-resident warps:
@@ -388,13 +387,13 @@ B2M_HD Affine<Fq> aff_add_slow(const Affine<Fq>& P, const Affine<Fq>& Q, uint32_
   return aff_finish(P, Q, true, den.inverse_fast(), &dummy);
 }
 
-// PHASE 0: both passes in one call.  PHASE 1 / 2: the split form -- two kernels per level.  What limits the fused kernel
-// (profiles/r02_level_kernel_notes.md): a single warp can issue an IMAD.WIDE only every ~6.5 cycles (the carry chains),
-// i.e. drive the multiplier to ~62 %, so the pipe is full only while >= 2 warps of a sub-partition are inside
-// multiplication code at the same time; the fused kernel's warps spend 40-60 % of their time elsewhere (operand
-// latency of the denominator pass, the ALU-only inversion) at 2-4 resident warps per sub-partition.  Split:
+// PHASE 0: both passes in one call.  PHASE 1 / 2: the split form -- two kernels per level.  What limits the fused kernel:
+// a single warp can issue a wide multiply only every few cycles (the carry chains), so the multiplier pipe is full only
+// while >= 2 warps of a sub-partition are inside multiplication code at the same time; the fused kernel's warps spend
+// much of their time elsewhere (operand latency of the denominator pass, the ALU-only inversion) at 2-4 resident warps
+// per sub-partition.  Split:
 //   PHASE 1 = denominator pass + inversion: ~90 registers, 5-6 CTAs/SM -- the gathers' latency and the inversions'
-//             ~27 k ALU instructions are spread over 5-6 warps per sub-partition instead of blocking a 128-168-register warp;
+//             tens of thousands of ALU instructions are spread over 5-6 warps per sub-partition instead of blocking a 128-168-register warp;
 //   PHASE 2 = addition pass only: every resident warp is inside multiplication code nearly all the time.
 // The chain inverse crosses in A.inv[t].
 //   PHASE 3 = denominator pass WITHOUT the inversion: the chain product goes to A.inv[t] and a separate kernel

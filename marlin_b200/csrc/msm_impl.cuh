@@ -135,7 +135,7 @@ static __global__ void msm_scatter_kernel(const uint32_t* digits, size_t n, size
 constexpr int MSM_Q = 64;      // nominal references per thread; the launch picks q near it so the grid is whole waves
 constexpr int MSM_Q_MIN = 32;  // buffers are sized for at least this many references per thread
 template <class Fq>
-__global__ void __launch_bounds__(128)  // 178 registers, 2 CTAs/SM; forcing 3 CTAs/SM (168 regs + spills) measured 5 % slower
+__global__ void __launch_bounds__(128)  // 2 CTAs/SM; forcing 3 CTAs/SM costs spills and was slower
 msm_accumulate_kernel(const Affine<Fq>* __restrict__ tables, size_t table_stride, const uint32_t* __restrict__ offsets,
                       const uint32_t* __restrict__ ends, const uint2* __restrict__ sorted, const uint32_t* __restrict__ total_refs_p,
                       const uint32_t q, XYZZ<Fq>* __restrict__ buckets, XYZZ<Fq>* __restrict__ part_pt,
@@ -334,8 +334,8 @@ msm_stitch_kernel(const XYZZ<Fq>* part_pt, const uint32_t* part_bkt, size_t nthr
 // shard of a 2^20 key picks -- ALL references of that window land in eight buckets of n / 8 references, each cut into
 // thousands of partials).  One WARP per queued entry: the lanes stride over the entry's slots, then a 5-step tree through
 // shared memory; runs of more than MSM_RUN_CHUNK slots were queued as chunks whose sums a second launch (FINAL) adds up.
-// (Round 1 folded runs of up to 256 slots serially in one thread -- 256 dependent XYZZ additions, ~2 ms of latency per
-// MSM -- and longer ones in one block each: `msm_stitch` grew from 1.3 ms to 8-13 ms per proof on 4 and 8 GPUs.)
+// (Folding runs of up to 256 slots serially in one thread -- 256 dependent XYZZ additions -- and longer ones in one block
+// each made the stitch several times slower on 4 and 8 GPUs.)
 // short runs: one thread per run, all lanes busy
 template <class Fq>
 __global__ void __launch_bounds__(128)
@@ -392,12 +392,12 @@ msm_stitch_runs_kernel(const XYZZ<Fq>* part_pt, const uint32_t* part_bkt, const 
 //     Rsum[hi] = sum_lo B[hi][lo]  (row tree),   Csum[lo] = sum_hi B[hi][lo]  (column tree),
 // and each of the two short weighted sums is done by bit planes: sum_i i V_i = sum_k 2^k sum_{i: bit k} V_i.
 
-// Both trees in two launches each, shaped for LATENCY as much as throughput (an XYZZ addition is ~9 us of dependent
+// Both trees in two launches each, shaped for LATENCY as much as throughput (an XYZZ addition is a long chain of dependent
 // multiplications, and the reduction sits on the critical path of every round: the host needs the commitments to draw the next
 // challenges).  Stage 1: one thread per (position, segment) adds K = 8 consecutive summands serially -- this is where the 2^19
 // buckets are read, one pass per axis.  Stage 2: one WARP per position folds the remaining len / 8 partials (strided loads, then a
-// 5-level tree through shared memory), rows and columns in the same launch.  Depth: 8 + <= 4 + 5 additions per tree (round 1's
-// pairwise kernels: 10 launches per tree; a 3-stage serial variant: 36 additions deep).
+// 5-level tree through shared memory), rows and columns in the same launch.  Depth: 8 + <= 4 + 5 additions per tree (pairwise
+// kernels would take 10 launches per tree; a 3-stage serial variant is 36 additions deep).
 //     stage 1: out[(g * ni + i) * nseg + s] = sum_{k < K} in[g * group_stride + (s * K + k) * stride_k + i * stride_i]
 template <class Fq>
 __global__ void __launch_bounds__(128) msm_segsum_kernel(const XYZZ<Fq>* __restrict__ in, XYZZ<Fq>* __restrict__ out, size_t groups, size_t nseg,
@@ -622,8 +622,7 @@ __global__ void g1_canonical_kernel(const Affine<Fq>* in, size_t n, Affine<Fq>* 
 template <class Fr, class Fq>
 int Msm<Fr, Fq>::pick_window(size_t n) {
   // n = powers of this key resident on ONE GPU.  The bucket pass costs n * ceil(256 / c) additions per MSM, the reduction
-  // ~0.8 ns per bucket plus a latency floor; measured (profiles/r02_scaling_notes.md, 2^20-constraint proofs and their per-rank
-  // equivalents): c = 20 (13 windows, 2^19 buckets) wins from 2^21 powers per GPU on, c = 16 (16 windows, 2^15 buckets, a full
+  // a fixed cost per bucket plus a latency floor; on 2^20-constraint proofs and their per-rank equivalents c = 20 (13 windows, 2^19 buckets) wins from 2^21 powers per GPU on, c = 16 (16 windows, 2^15 buckets, a full
   // top window) below that -- 4 and 8 GPUs on a 2^22-power key, or a single GPU on a small one -- and c ~ log2(n) - 1 for tiny keys.
   int lg = 0;
   while (((size_t)1 << (lg + 1)) <= n) lg++;
@@ -877,7 +876,7 @@ void Msm<Fr, Fq>::run_batch(const MsmJob<Fr, Fq>* jobs_in, int nj) {
             msm_affine_plan_kernel<Fq, false><<<div_up(nthreads, 256), 256, 0, cx.stream>>>(A);
           const Affine<Fq>* base = l == 0 ? tables.p : lvl_pts[(l - 1) & 1].p;
           const unsigned grid = div_up(nthreads, 128);
-          // Kernel variant (B2M_MSM_AFFINE_CTAS / _UPPER; every variant gives the same bytes, profiles/r02_level_kernel_notes.md):
+          // Kernel variant (B2M_MSM_AFFINE_CTAS / _UPPER; every variant gives the same bytes):
           //   4 (default), 5: fused kernel, loads at use, compiled for that many resident CTAs per SM; 3: operands prefetched (3 CTAs/SM)
           //   8, 9: fused, branch-free and software-pipelined addition pass (3 / 2 CTAs/SM)
           //   11-13: split -- denominator pass + inversion at 5 CTAs/SM, then the addition pass pipelined at 3 / 2 CTAs/SM or plain at 4

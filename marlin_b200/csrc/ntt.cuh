@@ -1,4 +1,4 @@
-// Radix-2 number-theoretic transform over Fr for sm_100a.
+// Radix-2 number-theoretic transform over Fr for sm_90a.
 //
 // Replaces ark-poly 0.3 `Radix2EvaluationDomain::{fft,ifft}_in_place` [U ark-poly
 // src/domain/radix2] behind every `domain.fft / ifft / interpolate /

@@ -357,8 +357,8 @@ struct MarlinIndex : IndexBase {
   // A group of INDEPENDENT transforms of one round.  One GPU: run them in order.  Several GPUs (the prover is replicated, so
   // every rank holds every input): transform j is computed by rank j mod world only and its result broadcast over NVLink --
   // north_star keeps a single NTT on one GPU, but a round's independent transforms need not all run on the same one.  Worth it
-  // for large transforms only (>= 2^24 points: at 2^24 constraints on 8 GPUs the NTTs are the largest term of the proof and
-  // sharing cut them from 319 to 182 + 58 ms of broadcasts); results are bit-identical either way.
+  // for large transforms only (>= 2^24 points: at 2^24 constraints on 8 GPUs the NTTs are the largest term of the proof);
+  // results are bit-identical either way.
   struct NttJob {
     const Fr* coeffs;  // padded form: `len` coefficients zero-extended to 2^log_n (work == nullptr)
     size_t len;
@@ -367,7 +367,7 @@ struct MarlinIndex : IndexBase {
     int log_n;
     bool inverse;
   };
-  int ntt_share_min_log = 24;  // measured (profiles/r02_scaling_notes.md): sharing 2^22-point transforms across 8 GPUs costs more in rank skew than it saves
+  int ntt_share_min_log = 24;  // sharing 2^22-point transforms across 8 GPUs costs more in rank skew than it saves
   void run_ntt_group(const std::vector<NttJob>& jobs) {
     const bool share = cx.world > 1 && cx.comm != nullptr && jobs.size() > 1 && jobs[0].log_n >= ntt_share_min_log;
     for (size_t j = 0; j < jobs.size(); j++) {

@@ -25,7 +25,7 @@ def test_every_declared_symbol_is_exported():
 
 def test_version_and_error_paths_without_gpu():
     L = _lib.lib()
-    assert b"sm_100a" in L.b2m_version()
+    assert b"sm_90a" in L.b2m_version()
     h = ctypes.c_void_p()
     import torch
     if not torch.cuda.is_available():

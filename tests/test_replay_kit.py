@@ -1,4 +1,4 @@
-"""CPU: the committed replay kit (tests/golden/replay_kit, written on a B200 by tools/make_replay_kit.py and consumed by
+"""CPU: the committed replay kit (tests/golden/replay_kit, written on a GPU by tools/make_replay_kit.py and consumed by
 tools/replay_rs on a machine with Rust) against the oracle: the GPU-made index_vk bytes and proof bytes are the oracle's for the same
 SRS, circuit and rng seed; the SRS file holds the oracle's G1 powers in `serialize_uncompressed` form and a consistent G2 half; and the
 bench.py reference arm keeps its JSON contract."""

@@ -1,6 +1,6 @@
 // Register-only ceilings of the batched-affine level arithmetic (no memory traffic): how fast can the addition pass, the
 // denominator pass and the inversion run on the whole chip at 1..4 resident CTAs (of 128 threads) per SM?
-// Compares with tools/microbench.cu's chained Fq multiplication (30.4 G/s) and XYZZ mixed addition (2.9 G/s).
+// Compares with tools/microbench.cu's chained Fq multiplication and XYZZ mixed addition rates.
 #include <cstdio>
 #include <cuda_runtime.h>
 #include "../marlin_b200/csrc/msm_affine.cuh"
