@@ -19,6 +19,10 @@ pub struct b2m_ck {
     _p: [u8; 0],
 }
 #[repr(C)]
+pub struct b2m_vk {
+    _p: [u8; 0],
+}
+#[repr(C)]
 pub struct b2m_matrix {
     pub row_ptr: *const u64,
     pub col: *const u64,
@@ -100,4 +104,15 @@ extern "C" {
     pub fn b2m_index_comms(idx: *const b2m_index, out_xy: *mut u64) -> c_int;
     pub fn b2m_prove(idx: *mut b2m_index, formatted_input: *const u64, n_input: usize, witness: *const u64, n_witness: usize,
                      zk_rng: *mut b2m_rng, proof: *mut u8, cap: usize, proof_len: *mut usize) -> c_int;
+
+    pub fn b2m_vk_create(ctx: *mut b2m_ctx, curve: c_int, pc_variant: c_int, num_constraints: usize, num_variables: usize,
+                         num_non_zero: usize, index_comms_xy: *const u64, g_xy: *const u64, gamma_g_xy: *const u64, h_bytes: *const u8,
+                         beta_h_bytes: *const u8, n_bounds: usize, bounds: *const u64, bound_points: *const c_void,
+                         out: *mut *mut b2m_vk) -> c_int;
+    pub fn b2m_vk_destroy(vk: *mut b2m_vk);
+    pub fn b2m_verify_batch(vk: *mut b2m_vk, n: usize, public_inputs: *const *const u64, n_inputs: *const usize,
+                            proofs: *const *const u8, proof_lens: *const usize, rng: *mut b2m_rng, verdicts: *mut c_int) -> c_int;
+    pub fn b2m_verify(vk: *mut b2m_vk, public_input: *const u64, n_input: usize, proof: *const u8, proof_len: usize,
+                      rng: *mut b2m_rng, ok: *mut c_int) -> c_int;
+    pub fn b2m_verify_timings(vk: *const b2m_vk, json: *mut c_char, cap: usize) -> c_int;
 }

@@ -267,6 +267,41 @@ int b2m_index_stage(b2m_index* idx, const uint64_t* formatted_input, size_t n_in
  * with the reference's own timer names (ark_std start_timer! labels, SURVEY.md section 5). */
 int b2m_prove_timings(const b2m_index* idx, char* json, size_t cap);
 
+/* ---- Level 2: verifier ABI -------------------------------------------------------------- */
+
+/* `IndexVerifierKey` plus the verifier half of the trimmed SRS (reference src/lib.rs:315-433 reads both), built from public
+ * data only.  The key borrows the context (destroy the key first, or the context is freed with its last child).
+ *   index_comms_xy : the six index commitments (row, col, a_val, b_val, c_val, row_col), affine x||y Montgomery
+ *   g_xy, gamma_g_xy : powers_of_g[0] and powers_of_gamma_g[0] of the SRS
+ *   h_bytes, beta_h_bytes : G2 points as ark-serialize uncompressed bytes (the b2m_g2_scalar_muls / SRS-file form),
+ *                    checked to be finite points of the curve
+ *   bounds[n_bounds] : the enforced degree bounds; they must include |H| - 2 and |K| - 2 of this index
+ *   bound_points   : per bound, MarlinKZG10: the G1 shift power powers_of_g[D - bound] (x||y Montgomery limbs, D = the SRS
+ *                    max degree); SonicKZG10: neg_powers_of_h[D - bound] = beta^-(D - bound) h (uncompressed G2 bytes)
+ * Errors: B2M_ERR_NON_SQUARE (num_constraints != num_variables), B2M_ERR_INVALID_ARG. */
+typedef struct b2m_vk b2m_vk;
+int b2m_vk_create(b2m_ctx* ctx, int curve, int pc_variant, size_t num_constraints, size_t num_variables, size_t num_non_zero,
+                  const uint64_t* index_comms_xy, const uint64_t* g_xy, const uint64_t* gamma_g_xy, const uint8_t* h_bytes,
+                  const uint8_t* beta_h_bytes, size_t n_bounds, const uint64_t* bounds, const void* bound_points, b2m_vk** out);
+void b2m_vk_destroy(b2m_vk* vk);
+
+/* `Marlin::verify` (reference src/lib.rs:315-433) for n proofs under one key.  public_inputs[i]: n_inputs[i] Montgomery Fr
+ * (the unformatted input, as Marlin::verify takes it); proofs[i]: proof_lens[i] `CanonicalSerialize` bytes of `Proof<F, PC>`.
+ * verdicts[i] = 1 accepted, 0 rejected by the check, -1 malformed bytes (framing, trailing bytes, x >= p, a point not on the
+ * curve or outside the prime-order subgroup, an evaluation or random_v >= r).  Malformed proofs are verdicts, not errors.
+ * The proofs' G1 points are decoded on the GPU; all checks of the batch are folded with one 128-bit randomiser per (proof,
+ * opening point) drawn from rng (which must be unpredictable to the prover) into a few MSMs on the GPU and one pairing
+ * product on the host; a failing batch is bisected with fresh randomisers until every bad proof is isolated.
+ * rng == NULL fails with B2M_ERR_MISSING_RNG. */
+int b2m_verify_batch(b2m_vk* vk, size_t n, const uint64_t* const* public_inputs, const size_t* n_inputs,
+                     const uint8_t* const* proofs, const size_t* proof_lens, b2m_rng* rng, int* verdicts);
+/* A batch of one: *ok receives the verdict (1, 0 or -1). */
+int b2m_verify(b2m_vk* vk, const uint64_t* public_input, size_t n_input, const uint8_t* proof, size_t proof_len,
+               b2m_rng* rng, int* ok);
+/* Phase split of the last b2m_verify_batch on this key (host wall-clock milliseconds around synchronised work):
+ * {"decode_ms", "transcript_ms", "msm_tables_ms", "msm_ms", "pairing_ms", "first_check_ms", "bisection_ms", "checks", ...}. */
+int b2m_verify_timings(const b2m_vk* vk, char* json, size_t cap);
+
 #ifdef __cplusplus
 }
 #endif

@@ -97,6 +97,12 @@ def lib():
             L.b2m_index_stage.argtypes = [vp, vp, sz, vp, sz]
             L.b2m_prove.argtypes = [vp, vp, sz, vp, sz, P(Rng), vp, sz, P(sz)]
             L.b2m_prove_timings.argtypes = [vp, ctypes.c_char_p, sz]
+            L.b2m_vk_create.argtypes = [vp, ci, ci, sz, sz, sz, vp, vp, vp, vp, vp, sz, vp, vp, P(vp)]
+            L.b2m_vk_destroy.argtypes = [vp]
+            L.b2m_vk_destroy.restype = None
+            L.b2m_verify_batch.argtypes = [vp, sz, vp, vp, vp, vp, P(Rng), vp]
+            L.b2m_verify.argtypes = [vp, vp, sz, vp, sz, P(Rng), P(ci)]
+            L.b2m_verify_timings.argtypes = [vp, ctypes.c_char_p, sz]
         _lib = L
     return _lib
 

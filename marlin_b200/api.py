@@ -1,10 +1,11 @@
 """Host-side mirror of the reference's public API for the accelerated path:
-`Marlin::<F, PC, FS>::{universal_setup, index, prove}` [reference src/lib.rs:79-311] with
+`Marlin::<F, PC, FS>::{universal_setup, index, prove, verify}` [reference src/lib.rs:79-433] with
 F in {BLS12-381 Fr, BN254 Fr}, PC in {MarlinKZG10, SonicKZG10}, FS = SimpleHashFiatShamirRng<Blake2s, ChaChaRng>.
 Every call lands in libb2m.so (include/b2m.h); nothing here computes on the CPU beyond marshalling.
 
-`verify` is not accelerated and not shipped by this package (SURVEY.md section 8f-2); proofs are
-`CanonicalSerialize` bytes that the reference's `Marlin::verify` consumes.
+Proofs are `CanonicalSerialize` bytes, the form the reference's `Marlin::verify` consumes.  `Marlin.verify_batch` checks
+many proofs under one verifier key at once (G1 decoding and the folded MSMs on the GPU, a constant number of pairings per
+batch on the host); `Marlin.verify` is a batch of one.
 """
 import ctypes
 import json
@@ -164,6 +165,24 @@ class IndexProverKey:
     def close(self):
         if self.handle:
             _lib.lib().b2m_index_destroy(self.handle)
+            self.handle = None
+
+
+class VerifierKey:
+    """`IndexVerifierKey` + the verifier half of the SRS (b2m_vk), built by `Marlin.verifier_key` from public data."""
+
+    def __init__(self, ctx, handle, curve_id, pc):
+        self.ctx, self.handle, self.curve_id, self.pc = ctx, handle, curve_id, pc
+
+    def timings(self):
+        """Phase split (ms) of the last verify_batch: decode, transcript, MSM tables, MSMs, pairings, bisection."""
+        buf = ctypes.create_string_buffer(4096)
+        _lib.check(_lib.lib().b2m_verify_timings(self.handle, buf, 4096))
+        return json.loads(buf.value.decode() or "{}")
+
+    def close(self):
+        if self.handle:
+            _lib.lib().b2m_vk_destroy(self.handle)
             self.handle = None
 
 
@@ -371,6 +390,72 @@ class Marlin:
             _lib.check(L.b2m_prove(index_pk.handle, _lib.ptr(inst), len(inst), _lib.ptr(wit), len(wit), ctypes.byref(zk_rng.c), buf,
                                    2048, ctypes.byref(n)))
         return bytes(buf[:n.value])
+
+    # -- verify ----------------------------------------------------------------------------------------
+    def verifier_key(self, index_pk, srs):
+        """The verifier key of an index: index_info, the six index commitments, g and gamma g, and the verifier's shift
+        material for the bounds |H| - 2 and |K| - 2 -- MarlinKZG10: powers_of_g[D - d]; SonicKZG10: beta^-(D - d) h -- with
+        h, beta h from the SRS's trapdoor or from the file it was loaded from (as `UniversalSRS.save` takes them)."""
+        from . import srsfile
+        import struct
+        L = _lib.lib()
+        cid = self.curve_id
+        nv, nc, nnz = struct.unpack_from("<QQQ", index_pk.vk_bytes, 0)
+
+        def p2(n):
+            s = 1
+            while s < n:
+                s *= 2
+            return s
+        bounds = sorted({p2(nc) - 2, p2(nnz) - 2})
+        D = srs.max_degree
+        if srs.trapdoor is not None:
+            h, beta_h, neg = srsfile.g2_setup(cid, fields.FR_MODULUS[cid], srs.trapdoor[0], D, bounds)
+        elif srs.g2 is not None:
+            h, beta_h, neg = srs.g2
+        else:
+            raise ValueError("this SRS has no G2 half (neither a trapdoor nor a source file)")
+        powers = np.ascontiguousarray(srs.powers_limbs)
+        if self.pc == _lib.PC_MARLIN_KZG10:
+            bound_points = np.ascontiguousarray(np.stack([powers[D - d] for d in bounds]))
+        else:
+            missing = [d for d in bounds if D - d not in neg]
+            if missing:
+                raise ValueError(f"the SRS holds no neg_powers_of_h for the degree bounds {missing}")
+            bound_points = np.frombuffer(b"".join(neg[D - d] for d in bounds), dtype=np.uint8).copy()
+        gamma_g = np.ascontiguousarray(srs.gamma_limbs[list(srs.gamma_indices).index(0)])
+        hb = np.frombuffer(h, dtype=np.uint8).copy()
+        bhb = np.frombuffer(beta_h, dtype=np.uint8).copy()
+        b = np.asarray(bounds, dtype=np.uint64)
+        handle = ctypes.c_void_p()
+        _lib.check(L.b2m_vk_create(self.ctx.handle, cid, self.pc, nc, nv, nnz, _lib.ptr(np.ascontiguousarray(index_pk.index_comms)),
+                                   _lib.ptr(np.ascontiguousarray(powers[0])), _lib.ptr(gamma_g), _lib.ptr(hb), _lib.ptr(bhb), len(b),
+                                   _lib.ptr(b), _lib.ptr(bound_points), ctypes.byref(handle)))
+        return VerifierKey(self.ctx, handle, cid, self.pc)
+
+    def verify_batch(self, vk, public_inputs, proofs, rng):
+        """`Marlin::verify` [reference src/lib.rs:315-433] for many proofs under one key.  public_inputs[i]: the field
+        elements (Python ints) of proof i's public input, without the leading one; rng: the ZkRng / CallbackRng the batch
+        randomisers are drawn from (unpredictable to the prover).  Returns True (accepted) / False (rejected) / None
+        (malformed bytes) per proof."""
+        n = len(proofs)
+        if len(public_inputs) != n:
+            raise ValueError("one public input per proof")
+        r = fields.FR_MODULUS[self.curve_id]
+        ins = [np.ascontiguousarray(_lib.ints_to_limbs([fields.fr_to_mont(self.curve_id, v % r) for v in x], 4)) for x in public_inputs]
+        bufs = [np.frombuffer(bytes(p), dtype=np.uint8).copy() if len(p) else np.zeros(1, dtype=np.uint8) for p in proofs]
+        in_ptrs = (ctypes.c_void_p * max(n, 1))(*[a.ctypes.data for a in ins])
+        in_lens = (ctypes.c_size_t * max(n, 1))(*[len(a) for a in ins])
+        pr_ptrs = (ctypes.c_void_p * max(n, 1))(*[a.ctypes.data for a in bufs])
+        pr_lens = (ctypes.c_size_t * max(n, 1))(*[len(p) for p in proofs])
+        verdicts = (ctypes.c_int * max(n, 1))()
+        _lib.check(_lib.lib().b2m_verify_batch(vk.handle, n, in_ptrs, in_lens, pr_ptrs, pr_lens,
+                                               ctypes.byref(rng.c) if rng is not None else None, verdicts))
+        return [{1: True, 0: False}.get(verdicts[i]) for i in range(n)]
+
+    def verify(self, vk, public_input, proof_bytes, rng):
+        """`Marlin::verify` of one proof -> bool (malformed bytes are False)."""
+        return self.verify_batch(vk, [public_input], [proof_bytes], rng)[0] is True
 
     def stage(self, index_pk, r1cs):
         """Copy (x, w) into HBM ahead of time (device-resident timing in bench.py)."""

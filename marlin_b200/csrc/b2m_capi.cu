@@ -2,6 +2,7 @@
 // The prover-level entry points live in prover.cu.
 #include "capi_types.cuh"
 #include "prover.cuh"
+#include "verify.cuh"
 #include "comm.cuh"
 #include <algorithm>
 #include "g2_host.hpp"
@@ -474,6 +475,67 @@ int b2m_prove_timings(const b2m_index* idx, char* json, size_t cap) {
   return guard([&] {
     B2M_REQUIRE(idx && json && cap > 0, B2M_ERR_INVALID_ARG, "null argument");
     snprintf(json, cap, "%s", idx->impl->timings_json.c_str());
+  });
+}
+
+// ---- Level 2: verifier ----------------------------------------------------------------------------
+struct b2m_vk {
+  b2m_ctx* ctx;
+  std::unique_ptr<VerifierBase> impl;
+};
+
+int b2m_vk_create(b2m_ctx* ctx, int curve, int pc_variant, size_t num_constraints, size_t num_variables, size_t num_non_zero,
+                  const uint64_t* index_comms_xy, const uint64_t* g_xy, const uint64_t* gamma_g_xy, const uint8_t* h_bytes,
+                  const uint8_t* beta_h_bytes, size_t n_bounds, const uint64_t* bounds, const void* bound_points, b2m_vk** out) {
+  return guard([&] {
+    B2M_REQUIRE(ctx && index_comms_xy && g_xy && gamma_g_xy && h_bytes && beta_h_bytes && out && (n_bounds == 0 || (bounds && bound_points)),
+                B2M_ERR_INVALID_ARG, "null argument");
+    B2M_REQUIRE(curve == B2M_CURVE_BLS12_381 || curve == B2M_CURVE_BN254, B2M_ERR_INVALID_ARG, "unknown curve id");
+    B2M_REQUIRE(pc_variant == B2M_PC_MARLIN_KZG10 || pc_variant == B2M_PC_SONIC_KZG10, B2M_ERR_INVALID_ARG, "unknown PC variant");
+    B2M_REQUIRE(ctx->cx.world <= 1, B2M_ERR_UNSUPPORTED, "verification on a multi-GPU context");
+    ctx->cx.use();
+    const VkArgs a{pc_variant, num_constraints, num_variables, num_non_zero, index_comms_xy, g_xy, gamma_g_xy, h_bytes, beta_h_bytes,
+                   n_bounds, bounds, bound_points};
+    std::unique_ptr<b2m_vk> vk(new b2m_vk{ctx, nullptr});
+    vk->impl.reset(curve == B2M_CURVE_BLS12_381 ? make_verifier_bls(ctx->cx, a) : make_verifier_bn(ctx->cx, a));
+    *out = vk.release();
+    ctx->children++;
+  });
+}
+
+void b2m_vk_destroy(b2m_vk* vk) {
+  if (!vk) return;
+  b2m_ctx* ctx = vk->ctx;
+  ctx->cx.use();
+  cudaStreamSynchronize(ctx->cx.stream);
+  delete vk;
+  if (--ctx->children == 0 && ctx->dead) b2m_release_ctx(ctx);
+}
+
+int b2m_verify_batch(b2m_vk* vk, size_t n, const uint64_t* const* public_inputs, const size_t* n_inputs, const uint8_t* const* proofs,
+                     const size_t* proof_lens, b2m_rng* rng, int* verdicts) {
+  return guard([&] {
+    B2M_REQUIRE(vk && (n == 0 || (public_inputs && n_inputs && proofs && proof_lens && verdicts)), B2M_ERR_INVALID_ARG, "null argument");
+    B2M_REQUIRE(rng != nullptr, B2M_ERR_MISSING_RNG, "rng is required (the batch randomisers must be unpredictable to the prover)");
+    B2M_REQUIRE(rng->kind == B2M_RNG_CHACHA8 || rng->kind == B2M_RNG_CHACHA12 || rng->kind == B2M_RNG_CHACHA20 ||
+                    (rng->kind == B2M_RNG_CALLBACK && rng->next_u64 != nullptr),
+                B2M_ERR_MISSING_RNG, "unsupported rng kind %d", rng->kind);
+    for (size_t i = 0; i < n; i++) B2M_REQUIRE(public_inputs[i] || n_inputs[i] == 0, B2M_ERR_INVALID_ARG, "public input %zu is null", i);
+    vk->ctx->cx.use();
+    vk->impl->verify_batch(n, public_inputs, n_inputs, proofs, proof_lens, rng, verdicts);
+  });
+}
+
+int b2m_verify(b2m_vk* vk, const uint64_t* public_input, size_t n_input, const uint8_t* proof, size_t proof_len, b2m_rng* rng, int* ok) {
+  int rc = guard([&] { B2M_REQUIRE(ok != nullptr, B2M_ERR_INVALID_ARG, "null argument"); });
+  if (rc != B2M_OK) return rc;
+  return b2m_verify_batch(vk, 1, &public_input, &n_input, &proof, &proof_len, rng, ok);
+}
+
+int b2m_verify_timings(const b2m_vk* vk, char* json, size_t cap) {
+  return guard([&] {
+    B2M_REQUIRE(vk && json && cap > 0, B2M_ERR_INVALID_ARG, "null argument");
+    snprintf(json, cap, "%s", vk->impl->timings_json.c_str());
   });
 }
 

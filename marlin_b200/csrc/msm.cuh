@@ -76,8 +76,10 @@ struct Msm {
   DBuf<Affine<Fq>> tables;  // [W][stride]:  tables[w * stride + k] = 2^(c*w) * P_(k * world + rank)
 
   static int pick_window(size_t n);
-  // Upload the powers and build the window tables (key-load time).
-  Msm(Ctx& cx, const Affine<Fq>* host_powers, size_t n, const Affine<Fq>* host_extra, size_t n_extra_bases, int window_bits);
+  // Upload the powers and build the window tables (key-load time).  powers_on_device: `powers` is a device array (the
+  // verifier's decoded proof points), copied on the device; single-GPU contexts only.
+  Msm(Ctx& cx, const Affine<Fq>* powers, size_t n, const Affine<Fq>* host_extra, size_t n_extra_bases, int window_bits,
+      bool powers_on_device = false);
 
   // sum_i scalars[i] * powers[base_off + i] (+ the `extra` XYZZ terms) -> out_xyzz / out_affine on
   // the device.  `scalars` is a device array, Montgomery form if mont, canonical otherwise.

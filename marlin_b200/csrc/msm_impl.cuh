@@ -646,8 +646,10 @@ int Msm<Fr, Fq>::pick_window(size_t n) {
 }
 
 template <class Fr, class Fq>
-Msm<Fr, Fq>::Msm(Ctx& cx, const Affine<Fq>* host_powers, size_t n, const Affine<Fq>* host_extra, size_t n_extra_bases, int window_bits)
+Msm<Fr, Fq>::Msm(Ctx& cx, const Affine<Fq>* host_powers, size_t n, const Affine<Fq>* host_extra, size_t n_extra_bases, int window_bits,
+                 bool powers_on_device)
     : ctx(&cx), n_extra(n_extra_bases), n_srs_global(n) {
+  B2M_REQUIRE(!powers_on_device || cx.world <= 1, B2M_ERR_UNSUPPORTED, "device-resident bases on a multi-GPU context");
   // Multi-GPU: GPU r keeps only the powers i = r (mod world) -- every contiguous slice of the key, whatever its
   // offset and length, then splits evenly over the GPUs, and table memory and build time drop by `world`.
   tab_world = cx.world > 1 ? cx.world : 1;
@@ -660,7 +662,9 @@ Msm<Fr, Fq>::Msm(Ctx& cx, const Affine<Fq>* host_powers, size_t n, const Affine<
   W = (Fr::Params::BITS + 1 + c - 1) / c;
   B2M_REQUIRE(W <= 32, B2M_ERR_INVALID_ARG, "too many windows (%d)", W);
   tables = DBuf<Affine<Fq>>(cx, (size_t)W * stride);
-  if (tab_world == 1) {
+  if (powers_on_device) {
+    B2M_CUDA(cudaMemcpyAsync(tables.p, host_powers, n * sizeof(Affine<Fq>), cudaMemcpyDeviceToDevice, cx.stream));
+  } else if (tab_world == 1) {
     tables.upload(host_powers, n);
   } else if (n_srs) {
     DBuf<Affine<Fq>> all(cx, n);

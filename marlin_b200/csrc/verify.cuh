@@ -1,0 +1,34 @@
+// Curve-independent interface of the batched verifier (Level 2 of include/b2m.h: b2m_vk_*, b2m_verify*).
+#pragma once
+#include <string>
+#include <vector>
+
+#include "common.cuh"
+
+namespace b2m {
+
+struct VerifierBase {
+  virtual ~VerifierBase() {}
+  // `Marlin::verify` [reference src/lib.rs:315-433] for n proofs under this key; verdicts[i] = 1 / 0 / -1 (malformed)
+  virtual void verify_batch(size_t n, const uint64_t* const* public_inputs, const size_t* n_inputs, const uint8_t* const* proofs,
+                            const size_t* proof_lens, b2m_rng* rng, int* verdicts) = 0;
+  std::string timings_json;
+};
+
+struct VkArgs {
+  int pc;
+  size_t num_constraints, num_variables, num_non_zero;
+  const uint64_t* index_comms_xy;
+  const uint64_t* g_xy;
+  const uint64_t* gamma_g_xy;
+  const uint8_t* h_bytes;
+  const uint8_t* beta_h_bytes;
+  size_t n_bounds;
+  const uint64_t* bounds;
+  const void* bound_points;
+};
+
+VerifierBase* make_verifier_bls(Ctx& cx, const VkArgs& a);
+VerifierBase* make_verifier_bn(Ctx& cx, const VkArgs& a);
+
+}  // namespace b2m
