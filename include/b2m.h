@@ -39,7 +39,8 @@ enum {
   B2M_ERR_MISSING_RNG = 7,              /* [U ark-poly-commit Error::MissingRng] */
   B2M_ERR_CUDA = 8,
   B2M_ERR_NCCL = 9,
-  B2M_ERR_UNSUPPORTED = 10
+  B2M_ERR_UNSUPPORTED = 10,
+  B2M_ERR_SERIALIZATION = 11            /* [U ark-serialize SerializationError::InvalidData]: an invalid point in a byte stream */
 };
 
 enum { B2M_CURVE_BLS12_381 = 0, B2M_CURVE_BN254 = 1 };
@@ -134,6 +135,26 @@ int b2m_g2_scalar_muls(int curve, const uint8_t* h_uncompressed, const uint64_t*
 int b2m_srs_export_g1(b2m_srs* srs, size_t first, size_t n, uint8_t* out);
 int b2m_g1_from_uncompressed(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, uint64_t* out_xy);
 int b2m_g1_to_uncompressed(b2m_ctx* ctx, int curve, const uint64_t* points_xy, size_t n, uint8_t* out);
+
+/* Checked decoding of ark-serialize points, `CanonicalDeserialize::deserialize` (compressed != 0) or
+ * `deserialize_uncompressed` semantics [U ark-serialize / ark-ec 0.3]: the flag bits (both set is invalid), every coordinate
+ * below p, the curve equation (compressed: a square root exists, and the sign bit picks the root) and the prime-order
+ * subgroup (BLS12-381 G1 by the endomorphism test phi(P) = -u^2 P; G2 by r * Q = O; BN254 G1 has cofactor 1).  Runs on the
+ * GPU, one thread per point, in chunks of 2^18 points, so device memory stays bounded whatever n is.
+ *   G1: bytes = n * sizeof(Fq) (compressed) or n * 2 sizeof(Fq); out_xy = n affine Montgomery points (infinity = 0, 0).
+ *   G2: bytes = n * 2 sizeof(Fq) or n * 4 sizeof(Fq) (x = c0 || c1, flags in the top of the last byte); out_uncompressed =
+ *       n * 4 sizeof(Fq) canonical bytes, the form b2m_g2_scalar_muls writes and b2m_vk_create takes.
+ * An invalid point fails with B2M_ERR_SERIALIZATION; *bad_index receives the lowest invalid index and *bad_reason its cause
+ * (1 both flags set, 2 x >= p, 3 not on the curve, 4 not in the subgroup, 5 y >= p), and b2m_last_error() names both; the
+ * output is then incomplete.  On success *bad_index = n and *bad_reason = 0.  bad_index / bad_reason may be NULL. */
+int b2m_g1_decode_ark(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, int compressed, uint64_t* out_xy,
+                      size_t* bad_index, int* bad_reason);
+int b2m_g2_decode_ark(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, int compressed, uint8_t* out_uncompressed,
+                      size_t* bad_index, int* bad_reason);
+/* `CanonicalSerialize::serialize` (compressed) of G1 points given as affine Montgomery limbs (GPU), and of G2 points given as
+ * uncompressed canonical bytes (host: no square root is needed).  Infinity is written as zero coordinates + bit 6. */
+int b2m_g1_to_compressed(b2m_ctx* ctx, int curve, const uint64_t* points_xy, size_t n, uint8_t* out);
+int b2m_g2_to_compressed(int curve, const uint8_t* uncompressed, size_t n, uint8_t* out);
 
 /* The caller's `zk_rng: &mut R` / `rng: Option<&mut dyn RngCore>` (reference src/lib.rs:154,125).  Two forms:
  *  - kind = B2M_RNG_CHACHA8/12/20, the fast path for the generators the reference's tests and benches use

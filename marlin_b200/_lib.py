@@ -13,6 +13,10 @@ CURVE_BN254 = 1
 PC_MARLIN_KZG10 = 0
 PC_SONIC_KZG10 = 1
 RNG_CHACHA8, RNG_CHACHA12, RNG_CHACHA20 = 8, 12, 20
+ERR_SERIALIZATION = 11
+# per-point causes of B2M_ERR_SERIALIZATION (b2m_g1_decode_ark / b2m_g2_decode_ark)
+POINT_REASONS = {1: "both flag bits set", 2: "x is not below the field modulus", 3: "not on the curve", 4: "not in the prime-order subgroup",
+                 5: "y is not below the field modulus"}
 
 # (Fr u64 limbs, Fq u64 limbs) per curve id
 LIMBS = {CURVE_BLS12_381: (4, 6), CURVE_BN254: (4, 4)}
@@ -78,6 +82,10 @@ def lib():
         L.b2m_srs_export_g1.argtypes = [vp, sz, sz, vp]
         L.b2m_g1_from_uncompressed.argtypes = [vp, ci, vp, sz, vp]
         L.b2m_g1_to_uncompressed.argtypes = [vp, ci, vp, sz, vp]
+        L.b2m_g1_decode_ark.argtypes = [vp, ci, vp, sz, ci, vp, P(sz), P(ci)]
+        L.b2m_g2_decode_ark.argtypes = [vp, ci, vp, sz, ci, vp, P(sz), P(ci)]
+        L.b2m_g1_to_compressed.argtypes = [vp, ci, vp, sz, vp]
+        L.b2m_g2_to_compressed.argtypes = [ci, vp, sz, vp]
         L.b2m_pc_commit.argtypes = [vp, ci, sz, vp, vp, vp, vp, P(Rng), vp, vp, vp, vp, sz]
         L.b2m_pc_open.argtypes = [vp, ci, sz, vp, vp, vp, vp, vp, sz, ctypes.c_int64, vp, vp, vp, P(ci), vp]
         L.b2m_trim.argtypes = [vp, ci, sz, sz, vp, sz, P(vp)]

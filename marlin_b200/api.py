@@ -114,6 +114,7 @@ class UniversalSRS:
         self.powers_limbs, self.gamma_limbs, self.gamma_indices = powers_limbs, gamma_limbs, gamma_indices
         self.trapdoor = None  # (beta, gamma) of an insecure test SRS made by universal_setup / srs_from_trapdoor
         self.g2 = None        # (h, beta_h, {index: neg power}) as ark-serialize bytes when loaded from / written to a file
+        self.ark = None       # load_ark_srs: the whole file as decoded -- every gamma power and neg_powers_of_h (save_ark)
 
     def save(self, path, degree_bounds=()):
         """Write the SRS as an ark-serialize file (marlin_b200/srsfile.py).  The G2 half -- h, beta h and SonicKZG10's
@@ -136,6 +137,52 @@ class UniversalSRS:
         else:
             raise ValueError("this SRS has no G2 half (neither a trapdoor nor a source file)")
         srsfile.write_srs(path, self.curve_id, powers.tobytes(), gamma, h, beta_h, neg)
+
+    def save_ark(self, path, compressed=True, degree_bounds=()):
+        """Write the SRS as a raw arkworks `kzg10::UniversalParams` file (`serialize` or `serialize_uncompressed`, no header;
+        marlin_b200/srsfile.py::read_ark).  An SRS from load_ark_srs writes everything its file held, so loading and saving in
+        the same form reproduces the file byte for byte (the point at infinity, should a file hold one, is written with zero
+        coordinates).  Otherwise the gamma powers are those on the device and the G2 half is made as `save` makes it."""
+        from . import srsfile
+        L = _lib.lib()
+        cid = self.curve_id
+        g1, g2 = srsfile.point_sizes(cid, compressed)
+        ark = self.ark
+        if ark is not None:
+            gkeys, glimbs = ark["gamma_keys"], ark["gamma_limbs"]
+            h, beta_h, nkeys, neg = ark["h"], ark["beta_h"], ark["neg_keys"], ark["neg"]
+        else:
+            gkeys, glimbs = np.asarray(self.gamma_indices, dtype=np.uint64), np.ascontiguousarray(self.gamma_limbs)
+            order = np.argsort(gkeys, kind="stable")
+            gkeys, glimbs = gkeys[order], np.ascontiguousarray(glimbs[order])
+            if self.trapdoor is not None:
+                h, beta_h, negd = srsfile.g2_setup(cid, fields.FR_MODULUS[cid], self.trapdoor[0], self.max_degree, degree_bounds)
+            elif self.g2 is not None:
+                h, beta_h, negd = self.g2
+            else:
+                raise ValueError("this SRS has no G2 half (neither a trapdoor nor a source file)")
+            nkeys = np.asarray(sorted(negd), dtype=np.uint64)
+            neg = np.frombuffer(b"".join(negd[int(k)] for k in nkeys), dtype=np.uint8).reshape(len(nkeys), 4 * srsfile.fq_bytes(cid))
+            h, beta_h = np.frombuffer(h, dtype=np.uint8), np.frombuffer(beta_h, dtype=np.uint8)
+
+        def g1_bytes(limbs):
+            limbs = np.ascontiguousarray(limbs, dtype=np.uint64)
+            out = np.zeros(len(limbs) * g1, dtype=np.uint8)
+            conv = L.b2m_g1_to_compressed if compressed else L.b2m_g1_to_uncompressed
+            _lib.check(conv(self.ctx.handle, cid, _lib.ptr(limbs), len(limbs), _lib.ptr(out)))
+            return out
+
+        def g2_bytes(unc):
+            unc = np.ascontiguousarray(unc, dtype=np.uint8)
+            if not compressed:
+                return unc
+            n = unc.size // (2 * g2)
+            out = np.zeros(n * g2, dtype=np.uint8)
+            _lib.check(L.b2m_g2_to_compressed(cid, _lib.ptr(unc), n, _lib.ptr(out)))
+            return out
+
+        srsfile.write_ark(path, cid, compressed, g1_bytes(self.powers_limbs), gkeys, g1_bytes(glimbs), g2_bytes(h), g2_bytes(beta_h), nkeys,
+                          g2_bytes(neg).reshape(len(nkeys), g2))
 
     def close(self):
         if self.handle:
@@ -259,6 +306,70 @@ class Marlin:
         _lib.check(L.b2m_g1_from_uncompressed(self.ctx.handle, self.curve_id, _lib.ptr(np.ascontiguousarray(graw)), len(idx), _lib.ptr(gam)))
         srs = self.srs_from_points(powers, gam, idx, window_bits)
         srs.g2 = (d["h"], d["beta_h"], d["neg_powers"])
+        return srs
+
+    def load_ark_srs(self, path, compressed=True, degree_bounds=(), window_bits=0):
+        """Load a raw arkworks `kzg10::UniversalParams` file, as `UniversalParams::serialize` (compressed=True) or
+        `serialize_uncompressed` wrote it, with `deserialize` semantics: every point is decoded and validated on the GPU (flags,
+        coordinates below p, on the curve, in the prime-order subgroup), and the first invalid one raises B2MError
+        (B2M_ERR_SERIALIZATION) naming its field and index, e.g. `powers_of_g[1048573]: not in the prime-order subgroup`
+        (BTreeMap fields are indexed by key).  The device key receives the gamma powers `universal_setup(degree_bounds=...)`
+        would make -- indices 0, 1, 2 and D - d + {0, 1, 2} per bound d -- while the returned SRS keeps the whole file (every
+        gamma power, every G2 point, contiguous) for `verifier_key` and `save_ark`."""
+        from . import srsfile
+        L = _lib.lib()
+        cid = self.curve_id
+        lq = _lib.LIMBS[cid][1]
+        g1, g2 = srsfile.point_sizes(cid, compressed)
+        d = srsfile.read_ark(path, cid, compressed)
+
+        def bad(field, names, idx, reason):
+            raise _lib.B2MError(_lib.ERR_SERIALIZATION, f"{field}[{names(idx)}]: {_lib.POINT_REASONS.get(reason, 'invalid point')}")
+
+        def g1_decode(pts, field, names=int):
+            pts = np.ascontiguousarray(pts)
+            out = np.zeros((len(pts), 2 * lq), dtype=np.uint64)
+            bi, br = ctypes.c_size_t(0), ctypes.c_int(0)
+            rc = L.b2m_g1_decode_ark(self.ctx.handle, cid, _lib.ptr(pts.reshape(-1)), len(pts), int(compressed), _lib.ptr(out), ctypes.byref(bi),
+                                     ctypes.byref(br))
+            if rc == _lib.ERR_SERIALIZATION:
+                bad(field, names, bi.value, br.value)
+            _lib.check(rc)
+            return out
+
+        n = len(d["powers"])
+        if n < 1:
+            raise ValueError(f"{path}: powers_of_g is empty")
+        D = n - 1
+        powers = g1_decode(d["powers"], "powers_of_g")
+        gkeys = d["gamma_keys"]
+        gamma_all = g1_decode(d["gamma"], "powers_of_gamma_g", lambda i: int(gkeys[i]))
+        nkeys = d["neg_keys"]
+        g2_in = np.concatenate([d["h"].reshape(1, g2), d["beta_h"].reshape(1, g2), d["neg"].reshape(-1, g2)])
+        g2_out = np.zeros((len(g2_in), 4 * srsfile.fq_bytes(cid)), dtype=np.uint8)
+        bi, br = ctypes.c_size_t(0), ctypes.c_int(0)
+        rc = L.b2m_g2_decode_ark(self.ctx.handle, cid, _lib.ptr(g2_in.reshape(-1)), len(g2_in), int(compressed), _lib.ptr(g2_out), ctypes.byref(bi),
+                                 ctypes.byref(br))
+        if rc == _lib.ERR_SERIALIZATION:
+            i = bi.value
+            field, names = (("h", None), ("beta_h", None))[i] if i < 2 else ("neg_powers_of_h", lambda j: int(nkeys[j - 2]))
+            if names is None:
+                raise _lib.B2MError(rc, f"{field}: {_lib.POINT_REASONS.get(br.value, 'invalid point')}")
+            bad(field, names, i, br.value)
+        _lib.check(rc)
+        # the gamma powers the PC needs on the device
+        idx = {0, 1, 2}
+        for b in sorted(set(degree_bounds)):
+            idx |= {D - b + i for i in range(3) if 0 <= D - b + i <= D}
+        idx = sorted(idx)
+        pos = np.searchsorted(gkeys, np.asarray(idx, dtype=np.uint64))
+        missing = [k for k, p in zip(idx, pos) if p >= len(gkeys) or int(gkeys[p]) != k]
+        if missing:
+            raise ValueError(f"{path}: powers_of_gamma_g holds no entry for the indices {missing}")
+        srs = self.srs_from_points(powers, gamma_all[pos], idx, window_bits)
+        h, beta_h, neg = g2_out[0], g2_out[1], np.ascontiguousarray(g2_out[2:])
+        srs.g2 = (h.tobytes(), beta_h.tobytes(), srsfile.G2Points(nkeys, neg))
+        srs.ark = {"gamma_keys": gkeys, "gamma_limbs": gamma_all, "h": h, "beta_h": beta_h, "neg_keys": nkeys, "neg": neg}
         return srs
 
     def srs_from_points(self, powers_limbs, gamma_limbs, gamma_indices, window_bits=0):

@@ -1,0 +1,29 @@
+// Batch conversion of ark-serialize G1 / G2 points on the GPU (the SRS loader: b2m_g1_decode_ark, b2m_g2_decode_ark,
+// b2m_g1_to_compressed).  Definitions in ark_points_impl.cuh, instantiated per curve by inst_ark_{bls,bn}.cu.
+#pragma once
+#include "common.cuh"
+#include "field.cuh"
+
+namespace b2m {
+
+// Points are decoded in chunks of this many, so the device scratch stays bounded whatever the input size.
+constexpr size_t ARK_DECODE_CHUNK = (size_t)1 << 18;
+
+// The lowest-indexed invalid point of a batch: index == n when every point is valid; reason = a G1_* status (g1_decode.cuh).
+struct ArkBad {
+  size_t index;
+  int reason;
+};
+
+// n points in either form -> affine Montgomery limbs (x || y, infinity = 0, 0).  Stops at the first chunk holding an invalid
+// point; out_xy is then filled below that chunk only.
+template <class Fq>
+ArkBad g1_decode_ark(Ctx& cx, const uint8_t* bytes, size_t n, bool compressed, uint64_t* out_xy);
+// n points in either form -> uncompressed canonical bytes (4 * sizeof(Fq) each).
+template <class Fq>
+ArkBad g2_decode_ark(Ctx& cx, const uint8_t* bytes, size_t n, bool compressed, uint8_t* out);
+// affine Montgomery limbs -> compressed bytes (sizeof(Fq) each).
+template <class Fq>
+void g1_to_compressed(Ctx& cx, const uint64_t* points_xy, size_t n, uint8_t* out);
+
+}  // namespace b2m

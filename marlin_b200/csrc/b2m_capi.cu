@@ -6,6 +6,8 @@
 #include "comm.cuh"
 #include <algorithm>
 #include "g2_host.hpp"
+#include "ark_points.cuh"
+#include "g2_decode.cuh"
 
 namespace b2m {
 thread_local std::string g_last_error;
@@ -201,6 +203,58 @@ int b2m_g1_from_uncompressed(b2m_ctx* ctx, int curve, const uint8_t* bytes, size
     ctx->cx.use();
     if (curve == B2M_CURVE_BLS12_381) Msm<FrBls, FqBls>::g1_from_bytes(ctx->cx, bytes, n, out_xy);
     else if (curve == B2M_CURVE_BN254) Msm<FrBn, FqBn>::g1_from_bytes(ctx->cx, bytes, n, out_xy);
+    else throw Error(B2M_ERR_INVALID_ARG, "unknown curve id");
+  });
+}
+
+static int ark_fail(const ArkBad& bad, size_t* bad_index, int* bad_reason) {
+  if (bad_index) *bad_index = bad.index;
+  if (bad_reason) *bad_reason = bad.reason;
+  return bad.reason == G1_OK ? B2M_OK : B2M_ERR_SERIALIZATION;
+}
+int b2m_g1_decode_ark(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, int compressed, uint64_t* out_xy, size_t* bad_index,
+                      int* bad_reason) {
+  return guard([&] {
+    B2M_REQUIRE(ctx && ((bytes && out_xy) || n == 0), B2M_ERR_INVALID_ARG, "null argument");
+    B2M_REQUIRE(curve == B2M_CURVE_BLS12_381 || curve == B2M_CURVE_BN254, B2M_ERR_INVALID_ARG, "unknown curve id");
+    ctx->cx.use();
+    const ArkBad bad = n == 0 ? ArkBad{0, G1_OK}
+                     : curve == B2M_CURVE_BLS12_381 ? g1_decode_ark<FqBls>(ctx->cx, bytes, n, compressed != 0, out_xy)
+                                                    : g1_decode_ark<FqBn>(ctx->cx, bytes, n, compressed != 0, out_xy);
+    if (ark_fail(bad, bad_index, bad_reason) != B2M_OK)
+      throw Error(B2M_ERR_SERIALIZATION, fmt("G1 point %zu: %s", bad.index, point_status_name(bad.reason)));
+  });
+}
+int b2m_g2_decode_ark(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, int compressed, uint8_t* out_uncompressed, size_t* bad_index,
+                      int* bad_reason) {
+  return guard([&] {
+    B2M_REQUIRE(ctx && ((bytes && out_uncompressed) || n == 0), B2M_ERR_INVALID_ARG, "null argument");
+    B2M_REQUIRE(curve == B2M_CURVE_BLS12_381 || curve == B2M_CURVE_BN254, B2M_ERR_INVALID_ARG, "unknown curve id");
+    ctx->cx.use();
+    const ArkBad bad = n == 0 ? ArkBad{0, G1_OK}
+                     : curve == B2M_CURVE_BLS12_381 ? g2_decode_ark<FqBls>(ctx->cx, bytes, n, compressed != 0, out_uncompressed)
+                                                    : g2_decode_ark<FqBn>(ctx->cx, bytes, n, compressed != 0, out_uncompressed);
+    if (ark_fail(bad, bad_index, bad_reason) != B2M_OK)
+      throw Error(B2M_ERR_SERIALIZATION, fmt("G2 point %zu: %s", bad.index, point_status_name(bad.reason)));
+  });
+}
+int b2m_g1_to_compressed(b2m_ctx* ctx, int curve, const uint64_t* points_xy, size_t n, uint8_t* out) {
+  return guard([&] {
+    B2M_REQUIRE(ctx && ((points_xy && out) || n == 0), B2M_ERR_INVALID_ARG, "null argument");
+    ctx->cx.use();
+    if (n == 0) return;
+    if (curve == B2M_CURVE_BLS12_381) g1_to_compressed<FqBls>(ctx->cx, points_xy, n, out);
+    else if (curve == B2M_CURVE_BN254) g1_to_compressed<FqBn>(ctx->cx, points_xy, n, out);
+    else throw Error(B2M_ERR_INVALID_ARG, "unknown curve id");
+  });
+}
+int b2m_g2_to_compressed(int curve, const uint8_t* uncompressed, size_t n, uint8_t* out) {
+  return guard([&] {
+    B2M_REQUIRE((uncompressed && out) || n == 0, B2M_ERR_INVALID_ARG, "null argument");
+    if (curve == B2M_CURVE_BLS12_381)
+      for (size_t i = 0; i < n; i++) g2_compress<FqBls>(uncompressed + i * 4 * FqBls::N * 4, out + i * 2 * FqBls::N * 4);
+    else if (curve == B2M_CURVE_BN254)
+      for (size_t i = 0; i < n; i++) g2_compress<FqBn>(uncompressed + i * 4 * FqBn::N * 4, out + i * 2 * FqBn::N * 4);
     else throw Error(B2M_ERR_INVALID_ARG, "unknown curve id");
   });
 }

@@ -4,84 +4,16 @@
 // the same limb code as the device (field.cuh compiled for the host), written out in ark-serialize's uncompressed form so that
 // an SRS file made here can be loaded by arkworks (tools/replay_rs).
 //
-// Fq2 = Fq[u] / (u^2 + 1) for both supported curves; E'(Fq2): y^2 = x^3 + b' (the formulas below never need b').
+// Fq2 and the G2 group law live in g2.cuh (shared with the GPU's SRS decoder).
 #pragma once
 #include <cstdint>
 #include <cstring>
 #include <vector>
 
 #include "field.cuh"
+#include "g2.cuh"
 
 namespace b2m {
-
-template <class Fq>
-struct Fq2 {
-  Fq c0, c1;
-  static Fq2 zero() { return Fq2{Fq::zero(), Fq::zero()}; }
-  static Fq2 one() { return Fq2{Fq::one(), Fq::zero()}; }
-  bool is_zero() const { return c0.is_zero() && c1.is_zero(); }
-  bool operator==(const Fq2& o) const { return c0 == o.c0 && c1 == o.c1; }
-  friend Fq2 operator+(const Fq2& a, const Fq2& b) { return Fq2{a.c0 + b.c0, a.c1 + b.c1}; }
-  friend Fq2 operator-(const Fq2& a, const Fq2& b) { return Fq2{a.c0 - b.c0, a.c1 - b.c1}; }
-  friend Fq2 operator*(const Fq2& a, const Fq2& b) {  // Karatsuba, u^2 = -1
-    const Fq v0 = a.c0 * b.c0, v1 = a.c1 * b.c1;
-    return Fq2{v0 - v1, (a.c0 + a.c1) * (b.c0 + b.c1) - v0 - v1};
-  }
-  Fq2 sqr() const { return (*this) * (*this); }
-  Fq2 dbl() const { return Fq2{c0.dbl(), c1.dbl()}; }
-  Fq2 neg() const { return Fq2{c0.neg(), c1.neg()}; }
-  Fq2 inverse() const {  // (c0 - c1 u) / (c0^2 + c1^2)
-    const Fq n = (c0.sqr() + c1.sqr()).inverse();
-    return Fq2{c0 * n, (c1 * n).neg()};
-  }
-};
-
-template <class Fq>
-struct G2Jac {  // Jacobian: (X / Z^2, Y / Z^3); infinity: Z = 0
-  Fq2<Fq> X, Y, Z;
-  static G2Jac inf() { return G2Jac{Fq2<Fq>::one(), Fq2<Fq>::one(), Fq2<Fq>::zero()}; }
-  bool is_inf() const { return Z.is_zero(); }
-  G2Jac dbl() const {  // dbl-2009-l (a = 0)
-    if (is_inf()) return *this;
-    const Fq2<Fq> A = X.sqr(), B = Y.sqr(), C = B.sqr();
-    const Fq2<Fq> D = ((X + B).sqr() - A - C).dbl();
-    const Fq2<Fq> E = A.dbl() + A, F = E.sqr();
-    G2Jac r;
-    r.X = F - D.dbl();
-    r.Y = E * (D - r.X) - C.dbl().dbl().dbl();
-    r.Z = (Y * Z).dbl();
-    return r;
-  }
-  G2Jac add(const G2Jac& o) const {  // add-2007-bl
-    if (is_inf()) return o;
-    if (o.is_inf()) return *this;
-    const Fq2<Fq> Z1Z1 = Z.sqr(), Z2Z2 = o.Z.sqr();
-    const Fq2<Fq> U1 = X * Z2Z2, U2 = o.X * Z1Z1;
-    const Fq2<Fq> S1 = Y * o.Z * Z2Z2, S2 = o.Y * Z * Z1Z1;
-    if (U1 == U2) return S1 == S2 ? dbl() : inf();
-    const Fq2<Fq> H = U2 - U1, I = H.dbl().sqr(), J = H * I, rr = (S2 - S1).dbl(), V = U1 * I;
-    G2Jac r;
-    r.X = rr.sqr() - J - V.dbl();
-    r.Y = rr * (V - r.X) - (S1 * J).dbl();
-    r.Z = ((Z + o.Z).sqr() - Z1Z1 - Z2Z2) * H;
-    return r;
-  }
-  // canonical little-endian scalar of nlimbs 32-bit limbs
-  G2Jac mul(const uint32_t* k, int nlimbs) const {
-    G2Jac acc = inf();
-    for (int i = nlimbs - 1; i >= 0; i--)
-      for (int b = 31; b >= 0; b--) {
-        acc = acc.dbl();
-        if ((k[i] >> b) & 1u) acc = acc.add(*this);
-      }
-    return acc;
-  }
-  void to_affine(Fq2<Fq>* x, Fq2<Fq>* y) const {  // (finite points only)
-    const Fq2<Fq> zi = Z.inverse(), zi2 = zi.sqr();
-    *x = X * zi2;
-    *y = Y * zi2 * zi;
-  }
-};
 
 // `CanonicalSerialize::serialize_uncompressed` of a short-Weierstrass affine point over Fq2 [U ark-ec 0.3
 // short_weierstrass_jacobian.rs + ark-ff QuadExtField]: x.c0 || x.c1 || y.c0 || y.c1, canonical little-endian, with the
