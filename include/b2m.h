@@ -260,6 +260,9 @@ typedef struct {
  * (src/ahp/indexer.rs:151-234, src/ahp/constraint_systems.rs:125-262) + `PC::trim` +
  * commitment to the six index polynomials.  The matrices must already be padded/squared
  * (num_constraints == num_variables) as `make_matrices_square_for_indexer` leaves them.
+ * Rows need not be in column order.  num_instance_variables (the formatted input, leading one
+ * included) must be a power of two (B2M_ERR_INVALID_PUBLIC_INPUT_LEN) and may equal
+ * num_variables (no witness at all); a column index >= num_variables is B2M_ERR_INVALID_ARG.
  * vk_bytes receives `IndexVerifierKey::write` (ToBytes) output: index_info || index_comms. */
 int b2m_index_create(b2m_srs* srs, int pc_variant, size_t num_constraints, size_t num_variables,
                      size_t num_instance_variables, const b2m_matrix* a, const b2m_matrix* b,

@@ -132,8 +132,9 @@ struct MarlinIndex : IndexBase {
     B2M_REQUIRE(nc >= 1 && ni <= nv, B2M_ERR_INVALID_ARG, "bad dimensions");
     const int S = Fr::Params::TWO_ADICITY;
     log_h = log2_ceil(nc); log_x = log2_ceil(ni);
-    H = (size_t)1 << log_h; X = ni;
-    B2M_REQUIRE(X < H, B2M_ERR_INVALID_ARG, "|X| must be smaller than |H|");
+    H = (size_t)1 << log_h; X = ni;  // X <= nv = nc <= H
+    // |X| == |H| (only public inputs, no witness) is a valid index, as in the reference: every column is then an input
+    // column, so reindex() maps i -> i, w(X) is the constant rho_w and z(X) = rho_w v_X(X) + x(X).
 
     // joint matrix (sorted union of the column sets per row) [reference indexer.rs:83-102]
     std::vector<uint32_t> jr, jc;
