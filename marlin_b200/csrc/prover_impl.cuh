@@ -26,30 +26,112 @@
 namespace b2m {
 
 template <class Fr>
-struct LcTerms {  // out[i] = sum_t coef[t] * (i < len[t] ? src[t][i] : 0)
+struct LcTerms {  // out[i] = sum_t coef[t] * (off[t] <= i < off[t] + len[t] ? src[t][i - off[t]] : 0)
   static constexpr int MAX = 8;
   const Fr* src[MAX];
-  size_t len[MAX];
+  size_t off[MAX], len[MAX];
   Fr coef[MAX];
   int n = 0;
-  void add(const Fr* p, size_t l, const Fr& c) {
-    src[n] = p; len[n] = l; coef[n] = c; n++;
+  void add(const Fr* p, size_t l, const Fr& c, size_t o = 0) {
+    src[n] = p; off[n] = o; len[n] = l; coef[n] = c; n++;
   }
 };
+// `out` may be one of the sources if its offset is 0: every thread reads its element before it writes it
 template <class Fr>
 __global__ void lincomb_kernel(LcTerms<Fr> t, size_t n, Fr* out) {
   size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   if (i >= n) return;
   Fr acc = Fr::zero();
   for (int k = 0; k < t.n; k++)
-    if (i < t.len[k]) acc = acc + t.coef[k] * ld_fr(t.src[k] + i);
+    if (i >= t.off[k] && i - t.off[k] < t.len[k]) acc = acc + t.coef[k] * ld_fr(t.src[k] + (i - t.off[k]));
   st_fr(out + i, acc);
 }
+
+// The witness MSMs of one or more opening points [U marlin_pc open].  A point's witness is its plain witness scalars against
+// powers_of_g[0 ..), its hiding witness against the gamma powers and, for MarlinKZG10, one shifted witness per degree-bounded
+// polynomial against powers_of_g[D - bound ..].  Each shifted witness is only ever added to its point's witness and an MSM is
+// linear in its scalars, so a shifted witness whose slice overlaps the plain slice, or starts at most MERGE_GAP powers past
+// its end, is summed into the plain scalars: one MSM over the union of the slices.  A shifted witness farther away stays an
+// MSM of its own in an earlier batch, and its result enters the point's MSM as an `extra` term: merging it would widen the
+// plain MSM by up to D zero scalars for a small bounded polynomial under a large key.
+template <class Fr, class Fq>
+struct WitnessMsms {
+  struct Shifted {  // coef * src[i] pairs with powers_of_g[off + i], i < n
+    const Fr* src;
+    Fr coef;
+    size_t n, off;
+  };
+  // A zero scalar has no digits: it costs the counting sort a few bytes and the bucket pass nothing.  A separate MSM costs its
+  // own sort and bucket reduction, and a whole batch (with its host round trip) when no other separate MSM shares it.
+  static constexpr size_t MERGE_GAP = 1024;
+
+  Ctx& cx;
+  std::vector<MsmJob<Fr, Fq>> pre, fin;  // the separate shifted witnesses; one MSM per point
+  std::vector<DBuf<Fr>> keep_sc;
+  std::vector<DBuf<XYZZ<Fq>>> keep_pt;
+  explicit WitnessMsms(Ctx& c) : cx(c) {}
+
+  // plain[0 .. n) may be overwritten; hw against the gamma powers from slot gslot; the affine witness goes to out (device)
+  void add_point(Fr* plain, size_t n, std::vector<Shifted> shifted, const std::vector<Fr>& hw, size_t gslot, Affine<Fq>* out) {
+    std::sort(shifted.begin(), shifted.end(), [](const Shifted& a, const Shifted& b) { return a.off < b.off; });
+    std::vector<Shifted> merged, apart;
+    size_t end = n;
+    for (const Shifted& s : shifted) {
+      if (s.n == 0) continue;
+      if (s.off <= end + MERGE_GAP) {
+        merged.push_back(s);
+        end = std::max(end, s.off + s.n);
+      } else {
+        apart.push_back(s);
+      }
+    }
+    Fr* sc = plain;
+    if (end > n) {
+      keep_sc.emplace_back(cx, end);
+      sc = keep_sc.back().p;
+    }
+    constexpr size_t per_pass = LcTerms<Fr>::MAX - 1;
+    for (size_t at = 0; at < merged.size(); at += per_pass) {
+      LcTerms<Fr> lt;
+      if (at == 0) lt.add(plain, n, Fr::one());
+      else lt.add(sc, end, Fr::one());
+      for (size_t k = at; k < std::min(merged.size(), at + per_pass); k++) lt.add(merged[k].src, merged[k].n, merged[k].coef, merged[k].off);
+      launch_lincomb(lt, end, sc);
+    }
+    DBuf<XYZZ<Fq>> ex(cx, std::max<size_t>(apart.size(), 1));
+    for (size_t k = 0; k < apart.size(); k++) {
+      keep_sc.emplace_back(cx, apart[k].n);
+      LcTerms<Fr> lt;
+      lt.add(apart[k].src, apart[k].n, apart[k].coef);
+      launch_lincomb(lt, apart[k].n, keep_sc.back().p);
+      pre.push_back(MsmJob<Fr, Fq>{keep_sc.back().p, true, apart[k].n, apart[k].off, nullptr, 0, 0, nullptr, 0, ex.p + k, nullptr});
+    }
+    const Fr* hw_dev = nullptr;
+    if (!hw.empty()) {
+      keep_sc.emplace_back(cx, hw.size());
+      keep_sc.back().upload(hw.data(), hw.size());
+      hw_dev = keep_sc.back().p;
+    }
+    fin.push_back(MsmJob<Fr, Fq>{sc, true, end, 0, hw_dev, hw.size(), gslot, ex.p, (int)apart.size(), nullptr, out});
+    keep_pt.push_back(std::move(ex));
+  }
+  // the separate shifted witnesses first: their results are `extra` terms of the points' MSMs
+  void run(Msm<Fr, Fq>& msm) {
+    for (size_t at = 0; at < pre.size(); at += MSM_MAX_BATCH) msm.run_batch(pre.data() + at, (int)std::min<size_t>(MSM_MAX_BATCH, pre.size() - at));
+    for (size_t at = 0; at < fin.size(); at += MSM_MAX_BATCH) msm.run_batch(fin.data() + at, (int)std::min<size_t>(MSM_MAX_BATCH, fin.size() - at));
+  }
+
+ private:
+  void launch_lincomb(const LcTerms<Fr>& lt, size_t n_out, Fr* dst) {
+    lincomb_kernel<Fr><<<div_up(n_out, 256), 256, 0, cx.stream>>>(lt, n_out, dst);
+    B2M_CHECK_LAUNCH();
+    cx.launches++;
+  }
+};
 
 template <class Fr, class Fq>
 struct MarlinIndex : IndexBase {
   using Pt = Affine<Fq>;
-  using Xy = XYZZ<Fq>;
   static constexpr int LQ = Fq::N / 2;  // u64 limbs of Fq
   static constexpr int FQ_BYTES = Fq::N * 4;
 
@@ -768,11 +850,10 @@ struct MarlinIndex : IndexBase {
     const Fr ch_outer = marlin ? xp[2] : xp[1], ch_t = marlin ? xp[3] : xp[2], ch_zb = marlin ? xp[4] : xp[3];
     const Fr ch_inner = marlin ? xp[2] : xp[1];
     DBuf<Pt> w_out(cx, 2);
-    std::vector<MsmJob<Fr, Fq>> shifted_jobs, final_jobs;
+    WitnessMsms<Fr, Fq> wit(cx);
+    typedef typename WitnessMsms<Fr, Fq>::Shifted Shifted;
     HPoly r_beta;       // combined hiding randomness at beta
     HPoly sr_beta;      // shifted randomness (Marlin PC): xi * shifted_rand(g_1)
-    std::vector<DBuf<Fr>> keep_sc;
-    std::vector<DBuf<Xy>> keep_pt;
     {
       // point beta: labels g_1, outer_sumcheck, t, z_b
       DBuf<Fr> pbeta(cx, 3 * H), sbeta(cx, 3 * H);
@@ -793,31 +874,18 @@ struct MarlinIndex : IndexBase {
       hp_axpy(r_beta, ch_outer, r_outer);
       hp_axpy(r_beta, ch_zb, o_zb.rand);
       HPoly hw = hp_is_zero(r_beta) ? HPoly() : hp_div_linear(r_beta, beta);  // hiding witness r / (X - beta)
-      DBuf<Xy> ex(cx, 2);
-      int n_extra = 0;
+      std::vector<Shifted> shifted;
       if (marlin) {
         hp_axpy(sr_beta, xp[1], o_g1.shifted_rand);
         if (!hp_is_zero(o_g1.shifted_rand)) hp_axpy(hw, xp[1], hp_div_linear(o_g1.shifted_rand, beta));
         // shifted witness: xi * (g_1 / (X - beta)) against powers_of_g[D - (|H| - 2) ..]
-        DBuf<Fr> sw(cx, o_g1.len);
-        const Fr* ps = s_g1.p + 1; Fr* pd = sw.p; const Fr x1 = xp[1];
-        ew(cx, o_g1.len - 1, [=] __device__(size_t i) { st_fr(pd + i, ld_fr(ps + i) * x1); });
-        shifted_jobs.push_back(MsmJob<Fr, Fq>{sw.p, true, o_g1.len - 1, shifted_off(o_g1.bound), nullptr, 0, 0, nullptr, 0, ex.p + n_extra,
-                                              nullptr});
-        n_extra++;
-        keep_sc.push_back(std::move(sw));
+        shifted.push_back(Shifted{s_g1.p + 1, xp[1], o_g1.len - 1, shifted_off(o_g1.bound)});
       }
-      const Fr* hw_dev = nullptr;
-      if (!hw.empty()) {
-        keep_sc.emplace_back(cx, hw.size());
-        keep_sc.back().upload(hw.data(), hw.size());
-        hw_dev = keep_sc.back().p;
-      }
-      final_jobs.push_back(MsmJob<Fr, Fq>{sbeta.p + 1, true, 3 * H - 1, 0, hw_dev, hw.size(), srs->gamma_slot(0), ex.p, n_extra, nullptr,
-                                          w_out.p});
-      keep_pt.push_back(std::move(ex));
-      keep_sc.push_back(std::move(pbeta));
-      keep_sc.push_back(std::move(sbeta));
+      wit.add_point(sbeta.p + 1, 3 * H - 1, shifted, hw, srs->gamma_slot(0), w_out.p);
+      // Both buffers (and pg, sg below) live until the MSMs have run: released here, they left the stream-ordered pool in a
+      // state where later allocations of this phase intermittently blocked in cudaMallocAsync for up to 0.3 s (H100, 2^20).
+      wit.keep_sc.push_back(std::move(sbeta));
+      wit.keep_sc.push_back(std::move(pbeta));
     }
     {
       // point gamma: labels g_2, inner_sumcheck (nothing hiding)
@@ -833,24 +901,13 @@ struct MarlinIndex : IndexBase {
       lt.add(o_h2.p, o_h2.len, ch_inner * ci_h2);
       lincomb(lt, K, pg.p);
       rec_suffix<Fr>(cx, pg.p, sg.p, K, 1, gamma, true);
-      DBuf<Xy> ex(cx, 1);
-      int n_extra = 0;
-      if (marlin) {
-        DBuf<Fr> sw(cx, o_g2.len);
-        const Fr* ps = s_g2.p + 1; Fr* pd = sw.p; const Fr x1 = xp[1];
-        ew(cx, o_g2.len - 1, [=] __device__(size_t i) { st_fr(pd + i, ld_fr(ps + i) * x1); });
-        shifted_jobs.push_back(MsmJob<Fr, Fq>{sw.p, true, o_g2.len - 1, shifted_off(o_g2.bound), nullptr, 0, 0, nullptr, 0, ex.p, nullptr});
-        n_extra = 1;
-        keep_sc.push_back(std::move(sw));
-      }
-      final_jobs.push_back(MsmJob<Fr, Fq>{sg.p + 1, true, K - 1, 0, nullptr, 0, 0, ex.p, n_extra, nullptr, w_out.p + 1});
-      keep_pt.push_back(std::move(ex));
-      keep_sc.push_back(std::move(pg));
-      keep_sc.push_back(std::move(sg));
+      std::vector<Shifted> shifted;
+      if (marlin) shifted.push_back(Shifted{s_g2.p + 1, xp[1], o_g2.len - 1, shifted_off(o_g2.bound)});
+      wit.add_point(sg.p + 1, K - 1, shifted, HPoly(), 0, w_out.p + 1);
+      wit.keep_sc.push_back(std::move(sg));
+      wit.keep_sc.push_back(std::move(pg));
     }
-    // the shifted parts feed the final points as `extra` terms, so they form their own (earlier) batch
-    if (!shifted_jobs.empty()) msm.run_batch(shifted_jobs.data(), (int)shifted_jobs.size());
-    msm.run_batch(final_jobs.data(), (int)final_jobs.size());
+    wit.run(msm);
     Pt w_pts[2];
     w_out.download(w_pts, 2);
     tm.end(t_op);
@@ -1026,9 +1083,9 @@ template <class Fr, class Fq>
 void pc_open_point_dev(b2m_srs* srs, Msm<Fr, Fq>& msm, int pc, const std::vector<OpenItem<Fr>>& items, int64_t max_degree_bound, const Fr& z,
                        const Fr& xi, uint64_t* out_w_xy, int* out_has_random_v, uint64_t* out_random_v) {
   using Pt = Affine<Fq>;
-  using Xy = XYZZ<Fq>;
   using M = MarlinIndex<Fr, Fq>;
   typedef typename M::HPoly HPoly;
+  typedef typename WitnessMsms<Fr, Fq>::Shifted Shifted;
   Ctx& cx = srs->ctx->cx;
   const size_t D = srs->n_g - 1;
   const bool marlin = pc == B2M_PC_MARLIN_KZG10;
@@ -1038,9 +1095,7 @@ void pc_open_point_dev(b2m_srs* srs, Msm<Fr, Fq>& msm, int pc, const std::vector
   std::vector<DBuf<Fr>> keep;
   DBuf<Fr> comb(cx, max_len), tmp(cx, max_len);
   comb.zero();
-  std::vector<MsmJob<Fr, Fq>> shifted_jobs;
-  DBuf<Xy> ex(cx, items.size() + 1);
-  int n_extra = 0;
+  std::vector<Shifted> shifted;
   HPoly r, sr, srw;
   Fr ch = one;
   bool enforce = false;
@@ -1063,13 +1118,8 @@ void pc_open_point_dev(b2m_srs* srs, Msm<Fr, Fq>& msm, int pc, const std::vector
       if (len > 1) {
         // shifted witness ch1 * (p_i / (X - z)) against shifted_powers: powers_of_g[D - bound ..]
         keep.emplace_back(cx, len);
-        DBuf<Fr>& sfx_i = keep.back();
-        rec_suffix<Fr>(cx, it.dev, sfx_i.p, len, 1, z, true);
-        Fr* ps = sfx_i.p;
-        const Fr c1 = ch;
-        ew(cx, len - 1, [=] __device__(size_t k) { st_fr(ps + 1 + k, ld_fr(ps + 1 + k) * c1); });
-        shifted_jobs.push_back(MsmJob<Fr, Fq>{sfx_i.p + 1, true, len - 1, D - (size_t)it.bound, nullptr, 0, 0, nullptr, 0, ex.p + n_extra, nullptr});
-        n_extra++;
+        rec_suffix<Fr>(cx, it.dev, keep.back().p, len, 1, z, true);
+        shifted.push_back(Shifted{keep.back().p + 1, ch, len - 1, D - (size_t)it.bound});
       }
       M::hp_axpy(sr, ch, it.srand);
       if (!M::hp_is_zero(it.srand)) M::hp_axpy(srw, ch, M::hp_div_linear(it.srand, z));
@@ -1082,17 +1132,10 @@ void pc_open_point_dev(b2m_srs* srs, Msm<Fr, Fq>& msm, int pc, const std::vector
   const bool hiding = !M::hp_is_zero(r);
   HPoly hw = hiding ? M::hp_div_linear(r, z) : HPoly();
   if (marlin && enforce) M::hp_axpy(hw, one, srw);
-  const Fr* hw_dev = nullptr;
-  if (!hw.empty()) {
-    keep.emplace_back(cx, hw.size());
-    keep.back().upload(hw.data(), hw.size());
-    hw_dev = keep.back().p;
-  }
-  for (size_t at = 0; at < shifted_jobs.size(); at += MSM_MAX_BATCH)
-    msm.run_batch(shifted_jobs.data() + at, (int)std::min<size_t>(MSM_MAX_BATCH, shifted_jobs.size() - at));
   DBuf<Pt> w(cx, 1);
-  MsmJob<Fr, Fq> fin{sfx.p + 1, true, max_len - 1, 0, hw_dev, hw.size(), hw.empty() ? 0 : srs->gamma_slot(0), ex.p, n_extra, nullptr, w.p};
-  msm.run_batch(&fin, 1);
+  WitnessMsms<Fr, Fq> wit(cx);
+  wit.add_point(sfx.p + 1, max_len - 1, shifted, hw, hw.empty() ? 0 : srs->gamma_slot(0), w.p);
+  wit.run(msm);
   Pt hwp;
   w.download(&hwp, 1);
   memcpy(out_w_xy, &hwp, sizeof(hwp));
