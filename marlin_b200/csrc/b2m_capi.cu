@@ -345,12 +345,27 @@ int b2m_pc_open(b2m_srs* srs, int pc_variant, size_t n_polys, const uint64_t* co
     B2M_REQUIRE(pc_variant == B2M_PC_MARLIN_KZG10 || pc_variant == B2M_PC_SONIC_KZG10, B2M_ERR_INVALID_ARG, "unknown PC variant");
     B2M_REQUIRE(n_polys >= 1, B2M_ERR_INVALID_ARG, "no polynomials");
     srs->ctx->cx.use();
-    if (srs->curve == B2M_CURVE_BLS12_381)
-      pc_open_bls(srs, pc_variant, n_polys, coeffs, n_coeffs, degree_bounds, rands, shifted_rands, rand_stride, max_degree_bound, point,
-                  opening_challenge, out_w_xy, out_has_random_v, out_random_v);
+    // open_combinations with one coefficient-one combination per polynomial, all queried at the one point; null rands
+    // give empty randomness
+    const bool bls = srs->curve == B2M_CURVE_BLS12_381;
+    std::vector<int> hiding(n_polys, 1);
+    std::vector<size_t> term_off(n_polys + 1), lc(n_polys), at_point(n_polys, 0);
+    std::vector<int64_t> poly(n_polys);
+    std::vector<uint64_t> ones(4 * n_polys);
+    for (size_t i = 0; i < n_polys; i++) {
+      term_off[i + 1] = i + 1;
+      lc[i] = i;
+      poly[i] = (int64_t)i;
+      memcpy(&ones[4 * i], bls ? FrBls::one().l : FrBn::one().l, 32);
+    }
+    if (bls)
+      pc_open_combinations_bls(srs, pc_variant, max_degree_bound, n_polys, coeffs, n_coeffs, degree_bounds, hiding.data(), rands, shifted_rands,
+                               rand_stride, n_polys, term_off.data(), poly.data(), ones.data(), n_polys, lc.data(), at_point.data(), 1, point,
+                               opening_challenge, out_w_xy, out_has_random_v, out_random_v);
     else
-      pc_open_bn(srs, pc_variant, n_polys, coeffs, n_coeffs, degree_bounds, rands, shifted_rands, rand_stride, max_degree_bound, point,
-                 opening_challenge, out_w_xy, out_has_random_v, out_random_v);
+      pc_open_combinations_bn(srs, pc_variant, max_degree_bound, n_polys, coeffs, n_coeffs, degree_bounds, hiding.data(), rands, shifted_rands,
+                              rand_stride, n_polys, term_off.data(), poly.data(), ones.data(), n_polys, lc.data(), at_point.data(), 1, point,
+                              opening_challenge, out_w_xy, out_has_random_v, out_random_v);
   });
 }
 

@@ -12,12 +12,6 @@ void pc_commit_bls(b2m_srs* srs, int pc, size_t n_polys, const uint64_t* const* 
   pc_commit_impl<FrBls, FqBls>(srs, *srs->bls, pc, n_polys, coeffs, n_coeffs, degree_bounds, hiding_bounds, rng, out_comm_xy, out_shifted_xy, out_rand,
                              out_shifted_rand, rand_stride);
 }
-void pc_open_bls(b2m_srs* srs, int pc, size_t n_polys, const uint64_t* const* coeffs, const size_t* n_coeffs, const int64_t* degree_bounds,
-                 const uint64_t* rands, const uint64_t* shifted_rands, size_t rand_stride, int64_t max_degree_bound, const uint64_t* point,
-                 const uint64_t* opening_challenge, uint64_t* out_w_xy, int* out_has_random_v, uint64_t* out_random_v) {
-  pc_open_impl<FrBls, FqBls>(srs, srs->ctx->ntt_bls(), *srs->bls, pc, n_polys, coeffs, n_coeffs, degree_bounds, rands, shifted_rands, rand_stride,
-                           max_degree_bound, point, opening_challenge, out_w_xy, out_has_random_v, out_random_v);
-}
 void pc_open_combinations_bls(b2m_srs* srs, int pc, int64_t max_degree_bound, size_t n_polys, const uint64_t* const* coeffs, const size_t* n_coeffs,
                               const int64_t* degree_bounds, const int* hiding, const uint64_t* rands, const uint64_t* shifted_rands, size_t rand_stride,
                               size_t n_lcs, const size_t* lc_term_off, const int64_t* lc_poly, const uint64_t* lc_coeff, size_t n_queries,

@@ -34,16 +34,7 @@ void pc_commit_bn(b2m_srs* srs, int pc, size_t n_polys, const uint64_t* const* c
                   const int64_t* degree_bounds, const int64_t* hiding_bounds, b2m_rng* rng, uint64_t* out_comm_xy,
                   uint64_t* out_shifted_xy, uint64_t* out_rand, uint64_t* out_shifted_rand, size_t rand_stride);
 
-// `PC::open` at one point over host polynomials (Level 1 of include/b2m.h)
-void pc_open_bls(b2m_srs* srs, int pc, size_t n_polys, const uint64_t* const* coeffs, const size_t* n_coeffs, const int64_t* degree_bounds,
-                 const uint64_t* rands, const uint64_t* shifted_rands, size_t rand_stride, int64_t max_degree_bound, const uint64_t* point,
-                 const uint64_t* opening_challenge, uint64_t* out_w_xy, int* out_has_random_v, uint64_t* out_random_v);
-void pc_open_bn(b2m_srs* srs, int pc, size_t n_polys, const uint64_t* const* coeffs, const size_t* n_coeffs, const int64_t* degree_bounds,
-                const uint64_t* rands, const uint64_t* shifted_rands, size_t rand_stride, int64_t max_degree_bound, const uint64_t* point,
-                const uint64_t* opening_challenge, uint64_t* out_w_xy, int* out_has_random_v, uint64_t* out_random_v);
-
-
-// `PC::open_combinations` over host polynomials (Level 1 of include/b2m.h)
+// `PC::open_combinations` over host polynomials, and `PC::open` as its one-point case (Level 1 of include/b2m.h)
 void pc_open_combinations_bls(b2m_srs* srs, int pc, int64_t max_degree_bound, size_t n_polys, const uint64_t* const* coeffs, const size_t* n_coeffs,
                               const int64_t* degree_bounds, const int* hiding, const uint64_t* rands, const uint64_t* shifted_rands, size_t rand_stride,
                               size_t n_lcs, const size_t* lc_term_off, const int64_t* lc_poly, const uint64_t* lc_coeff, size_t n_queries,

@@ -18,6 +18,7 @@
 
 #include "capi_types.cuh"
 #include "hostutil.hpp"
+#include "pc_impl.cuh"
 #include "poly_impl.cuh"
 #include "prover.cuh"
 #include "comm.cuh"
@@ -25,113 +26,10 @@
 
 namespace b2m {
 
-template <class Fr>
-struct LcTerms {  // out[i] = sum_t coef[t] * (off[t] <= i < off[t] + len[t] ? src[t][i - off[t]] : 0)
-  static constexpr int MAX = 8;
-  const Fr* src[MAX];
-  size_t off[MAX], len[MAX];
-  Fr coef[MAX];
-  int n = 0;
-  void add(const Fr* p, size_t l, const Fr& c, size_t o = 0) {
-    src[n] = p; off[n] = o; len[n] = l; coef[n] = c; n++;
-  }
-};
-// `out` may be one of the sources if its offset is 0: every thread reads its element before it writes it
-template <class Fr>
-__global__ void lincomb_kernel(LcTerms<Fr> t, size_t n, Fr* out) {
-  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  Fr acc = Fr::zero();
-  for (int k = 0; k < t.n; k++)
-    if (i >= t.off[k] && i - t.off[k] < t.len[k]) acc = acc + t.coef[k] * ld_fr(t.src[k] + (i - t.off[k]));
-  st_fr(out + i, acc);
-}
-
-// The witness MSMs of one or more opening points [U marlin_pc open].  A point's witness is its plain witness scalars against
-// powers_of_g[0 ..), its hiding witness against the gamma powers and, for MarlinKZG10, one shifted witness per degree-bounded
-// polynomial against powers_of_g[D - bound ..].  Each shifted witness is only ever added to its point's witness and an MSM is
-// linear in its scalars, so a shifted witness whose slice overlaps the plain slice, or starts at most MERGE_GAP powers past
-// its end, is summed into the plain scalars: one MSM over the union of the slices.  A shifted witness farther away stays an
-// MSM of its own in an earlier batch, and its result enters the point's MSM as an `extra` term: merging it would widen the
-// plain MSM by up to D zero scalars for a small bounded polynomial under a large key.
-template <class Fr, class Fq>
-struct WitnessMsms {
-  struct Shifted {  // coef * src[i] pairs with powers_of_g[off + i], i < n
-    const Fr* src;
-    Fr coef;
-    size_t n, off;
-  };
-  // A zero scalar has no digits: it costs the counting sort a few bytes and the bucket pass nothing.  A separate MSM costs its
-  // own sort and bucket reduction, and a whole batch (with its host round trip) when no other separate MSM shares it.
-  static constexpr size_t MERGE_GAP = 1024;
-
-  Ctx& cx;
-  std::vector<MsmJob<Fr, Fq>> pre, fin;  // the separate shifted witnesses; one MSM per point
-  std::vector<DBuf<Fr>> keep_sc;
-  std::vector<DBuf<XYZZ<Fq>>> keep_pt;
-  explicit WitnessMsms(Ctx& c) : cx(c) {}
-
-  // plain[0 .. n) may be overwritten; hw against the gamma powers from slot gslot; the affine witness goes to out (device)
-  void add_point(Fr* plain, size_t n, std::vector<Shifted> shifted, const std::vector<Fr>& hw, size_t gslot, Affine<Fq>* out) {
-    std::sort(shifted.begin(), shifted.end(), [](const Shifted& a, const Shifted& b) { return a.off < b.off; });
-    std::vector<Shifted> merged, apart;
-    size_t end = n;
-    for (const Shifted& s : shifted) {
-      if (s.n == 0) continue;
-      if (s.off <= end + MERGE_GAP) {
-        merged.push_back(s);
-        end = std::max(end, s.off + s.n);
-      } else {
-        apart.push_back(s);
-      }
-    }
-    Fr* sc = plain;
-    if (end > n) {
-      keep_sc.emplace_back(cx, end);
-      sc = keep_sc.back().p;
-    }
-    constexpr size_t per_pass = LcTerms<Fr>::MAX - 1;
-    for (size_t at = 0; at < merged.size(); at += per_pass) {
-      LcTerms<Fr> lt;
-      if (at == 0) lt.add(plain, n, Fr::one());
-      else lt.add(sc, end, Fr::one());
-      for (size_t k = at; k < std::min(merged.size(), at + per_pass); k++) lt.add(merged[k].src, merged[k].n, merged[k].coef, merged[k].off);
-      launch_lincomb(lt, end, sc);
-    }
-    DBuf<XYZZ<Fq>> ex(cx, std::max<size_t>(apart.size(), 1));
-    for (size_t k = 0; k < apart.size(); k++) {
-      keep_sc.emplace_back(cx, apart[k].n);
-      LcTerms<Fr> lt;
-      lt.add(apart[k].src, apart[k].n, apart[k].coef);
-      launch_lincomb(lt, apart[k].n, keep_sc.back().p);
-      pre.push_back(MsmJob<Fr, Fq>{keep_sc.back().p, true, apart[k].n, apart[k].off, nullptr, 0, 0, nullptr, 0, ex.p + k, nullptr});
-    }
-    const Fr* hw_dev = nullptr;
-    if (!hw.empty()) {
-      keep_sc.emplace_back(cx, hw.size());
-      keep_sc.back().upload(hw.data(), hw.size());
-      hw_dev = keep_sc.back().p;
-    }
-    fin.push_back(MsmJob<Fr, Fq>{sc, true, end, 0, hw_dev, hw.size(), gslot, ex.p, (int)apart.size(), nullptr, out});
-    keep_pt.push_back(std::move(ex));
-  }
-  // the separate shifted witnesses first: their results are `extra` terms of the points' MSMs
-  void run(Msm<Fr, Fq>& msm) {
-    for (size_t at = 0; at < pre.size(); at += MSM_MAX_BATCH) msm.run_batch(pre.data() + at, (int)std::min<size_t>(MSM_MAX_BATCH, pre.size() - at));
-    for (size_t at = 0; at < fin.size(); at += MSM_MAX_BATCH) msm.run_batch(fin.data() + at, (int)std::min<size_t>(MSM_MAX_BATCH, fin.size() - at));
-  }
-
- private:
-  void launch_lincomb(const LcTerms<Fr>& lt, size_t n_out, Fr* dst) {
-    lincomb_kernel<Fr><<<div_up(n_out, 256), 256, 0, cx.stream>>>(lt, n_out, dst);
-    B2M_CHECK_LAUNCH();
-    cx.launches++;
-  }
-};
-
 template <class Fr, class Fq>
 struct MarlinIndex : IndexBase {
   using Pt = Affine<Fq>;
+  using LP = LabeledPoly<Fr, Fq>;
   static constexpr int LQ = Fq::N / 2;  // u64 limbs of Fq
   static constexpr int FQ_BYTES = Fq::N * 4;
 
@@ -151,7 +49,7 @@ struct MarlinIndex : IndexBase {
   DBuf<Fr> t_coeff;
   size_t t_entries = 0;
   DBuf<Fr> ipoly[6], ieval[6];  // row, col, a_val, b_val, c_val, row_col (coefficients / evaluations on K)
-  Pt index_comms[6];
+  LP index_polys[6];  // ipoly with their commitments
 
   struct Timer {
     Ctx& cx;
@@ -197,9 +95,6 @@ struct MarlinIndex : IndexBase {
     return r;
   }
   static bool is_pow2(size_t v) { return v && !(v & (v - 1)); }
-
-  // shifted_powers(bound) start at powers_of_g[D - bound]   [U marlin_pc / sonic_pc CommitterKey]
-  size_t shifted_off(size_t bound) const { return D - bound; }
 
   // ---------------------------------------------------------------------------------------------
   // `Marlin::index`: AHPForR1CS::index + trim + commit
@@ -331,18 +226,19 @@ struct MarlinIndex : IndexBase {
       cx.sync();
     }
     // commit to the index polynomials, rng = None [reference lib.rs:124-125]
-    {
-      DBuf<Pt> out(cx, 6);
-      MsmJob<Fr, Fq> jobs[6];
-      for (int i = 0; i < 6; i++) jobs[i] = MsmJob<Fr, Fq>{ipoly[i].p, true, K, 0, nullptr, 0, 0, nullptr, 0, nullptr, out.p + i};
-      msm.run_batch(jobs, 6);
-      out.download(index_comms, 6);
+    std::vector<LP*> ips;
+    for (int i = 0; i < 6; i++) {
+      index_polys[i].p = ipoly[i].p;
+      index_polys[i].len = K;
+      ips.push_back(&index_polys[i]);
     }
+    ZkSource<b2m_rng> no_rng(nullptr);
+    pc_commit(srs, msm, pc, ips, no_rng);
     comms_xy.resize(6 * 2 * LQ);
-    memcpy(comms_xy.data(), index_comms, sizeof(index_comms));
+    for (int i = 0; i < 6; i++) memcpy(comms_xy.data() + i * 2 * LQ, &index_polys[i].comm, sizeof(Pt));
     // IndexVerifierKey::write: index_info (3 x u64) || index_comms  [reference data_structures.rs:36-43, indexer.rs:63-69]
     put_u64(vk_bytes, nv); put_u64(vk_bytes, nc); put_u64(vk_bytes, nnz);
-    for (int i = 0; i < 6; i++) write_commitment(vk_bytes, index_comms[i], false, Pt::inf());
+    for (int i = 0; i < 6; i++) write_commitment(vk_bytes, index_polys[i].comm, false, Pt::inf());
   }
 
   // ---- ToBytes / CanonicalSerialize of group and field elements (SURVEY.md A.2 / A.3) ------------
@@ -388,33 +284,6 @@ struct MarlinIndex : IndexBase {
     if (y.canonical_gt_half()) out[at + FQ_BYTES - 1] |= 1 << 7;
   }
 
-  // ---- small host-side polynomials (the 3-coefficient KZG blinding polynomials) -------------------
-  typedef std::vector<Fr> HPoly;
-  static void hp_axpy(HPoly& acc, const Fr& k, const HPoly& p) {
-    if (acc.size() < p.size()) acc.resize(p.size(), Fr::zero());
-    for (size_t i = 0; i < p.size(); i++) acc[i] = acc[i] + k * p[i];
-  }
-  static Fr hp_eval(const HPoly& p, const Fr& z) {
-    Fr acc = Fr::zero();
-    for (size_t i = p.size(); i-- > 0;) acc = acc * z + p[i];
-    return acc;
-  }
-  static HPoly hp_div_linear(const HPoly& p, const Fr& z) {  // quotient of p / (X - z)
-    if (p.size() <= 1) return HPoly();
-    HPoly q(p.size() - 1);
-    Fr acc = Fr::zero();
-    for (size_t i = p.size() - 1; i >= 1; i--) {
-      acc = p[i] + acc * z;
-      q[i - 1] = acc;
-    }
-    return q;
-  }
-  static bool hp_is_zero(const HPoly& p) {
-    for (auto& c : p)
-      if (!c.is_zero()) return false;
-    return true;
-  }
-
   // ---- device helpers -----------------------------------------------------------------------------
   // c (|H| + 1 coefficients, c[|H|] not yet written) += rho * v_H    [reference prover.rs:350-366]
   void blind(Fr* c, Fr rho) {
@@ -423,11 +292,6 @@ struct MarlinIndex : IndexBase {
       if (i == 0) st_fr(c, ld_fr(c) - rho);
       else st_fr(c + Hh, rho);
     });
-  }
-  void lincomb(const LcTerms<Fr>& t, size_t n, Fr* out) {
-    lincomb_kernel<Fr><<<div_up(n, 256), 256, 0, cx.stream>>>(t, n, out);
-    B2M_CHECK_LAUNCH();
-    cx.launches++;
   }
   // forward NTT of `len` coefficients zero-extended to 2^log_n, result in `out` (2^log_n elements)
   void fft_padded(const Fr* coeffs, size_t len, int log_n, Fr* out) {
@@ -471,77 +335,9 @@ struct MarlinIndex : IndexBase {
     return h;
   }
 
-  // One KZG10::commit as an MSM job: powers_of_g[off..off+len) against the coefficients, and the blinding
-  // polynomial against the gamma powers starting at gamma slot `gslot` -- all in the same bucket pass.
-  MsmJob<Fr, Fq> kzg_commit_job(const Fr* coeffs, size_t len, size_t off, const HPoly& blinding, size_t gslot, Pt* out_dev,
-                                std::vector<DBuf<Fr>>& keep_sc) {
-    const Fr* s2 = nullptr;
-    if (!blinding.empty()) {
-      keep_sc.emplace_back(cx, blinding.size());
-      keep_sc.back().upload(blinding.data(), blinding.size());
-      s2 = keep_sc.back().p;
-    }
-    return MsmJob<Fr, Fq>{coeffs, true, len, off, s2, blinding.size(), gslot, nullptr, 0, nullptr, out_dev};
-  }
-
-  struct Oracle {       // a labelled polynomial living in HBM
-    const Fr* p = nullptr;
-    size_t len = 0;
-    bool bounded = false;
-    size_t bound = 0;
-    bool hiding = false;
-    HPoly rand, shifted_rand;  // kzg10::Randomness blinding polynomials (host)
-    Pt comm, shifted_comm;
-  };
-
-  // `PC::commit` over a round's oracles, drawing blinding polynomials from zk in the reference's order.
-  void commit_round(std::vector<Oracle*>& polys, ZkSource<b2m_rng>& zk) {
-    std::vector<DBuf<Fr>> keep_sc;
-    DBuf<Pt> out(cx, 2 * polys.size());
-    out.zero();  // the shifted slot of an unbounded polynomial is never written
-    std::vector<MsmJob<Fr, Fq>> jobs;
-    for (size_t i = 0; i < polys.size(); i++) {
-      Oracle& o = *polys[i];
-      auto draw = [&]() {
-        HPoly r;
-        if (o.hiding)
-          for (int k = 0; k < 3; k++) r.push_back(field_rand<Fr>(zk));  // degree hiding_bound + 1 = 2
-        return r;
-      };
-      if (pc == B2M_PC_MARLIN_KZG10) {
-        o.rand = draw();
-        jobs.push_back(kzg_commit_job(o.p, o.len, 0, o.rand, srs->gamma_slot(0), out.p + 2 * i, keep_sc));
-        if (o.bounded) {
-          o.shifted_rand = draw();
-          jobs.push_back(kzg_commit_job(o.p, o.len, shifted_off(o.bound), o.shifted_rand, srs->gamma_slot(0), out.p + 2 * i + 1, keep_sc));
-        }
-      } else {
-        o.rand = draw();
-        if (o.bounded)
-          jobs.push_back(kzg_commit_job(o.p, o.len, shifted_off(o.bound), o.rand, o.hiding ? sonic_gamma_slot(o.bound) : 0,
-                                        out.p + 2 * i, keep_sc));
-        else
-          jobs.push_back(kzg_commit_job(o.p, o.len, 0, o.rand, o.hiding ? srs->gamma_slot(0) : 0, out.p + 2 * i, keep_sc));
-      }
-    }
-    msm.run_batch(jobs.data(), (int)jobs.size());
-    std::vector<Pt> h(2 * polys.size());
-    out.download(h.data(), h.size());
-    for (size_t i = 0; i < polys.size(); i++) {
-      polys[i]->comm = h[2 * i];
-      polys[i]->shifted_comm = h[2 * i + 1];
-    }
-  }
-  // sonic_pc shifted_powers_of_gamma_g[bound]: powers max_degree - bound + {0, 1, 2} in consecutive slots
-  size_t sonic_gamma_slot(size_t bound) const {
-    size_t s0 = srs->gamma_slot(D - bound);
-    for (size_t i = 1; i < 3; i++)
-      B2M_REQUIRE(srs->gamma_slot(D - bound + i) == s0 + i, B2M_ERR_INVALID_ARG, "gamma powers for bound %zu are not consecutive", bound);
-    return s0;
-  }
-  void absorb_comms(FiatShamir& fs, std::vector<Oracle*>& polys) {
+  void absorb_comms(FiatShamir& fs, const std::vector<LP*>& polys) {
     std::vector<uint8_t> bytes;
-    for (auto* o : polys) write_commitment(bytes, o->comm, o->bounded && pc == B2M_PC_MARLIN_KZG10, o->shifted_comm);
+    for (auto* o : polys) write_commitment(bytes, o->comm, o->bound >= 0 && pc == B2M_PC_MARLIN_KZG10, o->shifted_comm);
     fs.absorb(bytes);
   }
   Fr sample_outside_h(FiatShamir& fs) {  // sample_element_outside_domain
@@ -581,10 +377,7 @@ struct MarlinIndex : IndexBase {
       n_input = ni;
       n_witness = nv - ni;
     }
-    B2M_REQUIRE(n_input + n_witness == nv, B2M_ERR_INSTANCE_MISMATCH, "instance (%zu + %zu variables) does not match the index (%zu)",
-                n_input, n_witness, nv);
-    B2M_REQUIRE(n_input == ni && is_pow2(n_input), B2M_ERR_INVALID_PUBLIC_INPUT_LEN, "formatted public input length %zu (index: %zu)",
-                n_input, ni);
+    check_instance(n_input, n_witness);
     B2M_REQUIRE(rng->kind == B2M_RNG_CHACHA8 || rng->kind == B2M_RNG_CHACHA12 || rng->kind == B2M_RNG_CHACHA20 ||
                     (rng->kind == B2M_RNG_CALLBACK && rng->next_u64 != nullptr),
                 B2M_ERR_MISSING_RNG, "unsupported rng kind %d", rng->kind);
@@ -651,11 +444,11 @@ struct MarlinIndex : IndexBase {
     Fr rho_w = field_rand<Fr>(zk), rho_a = field_rand<Fr>(zk), rho_b = field_rand<Fr>(zk);
     blind(wt.p, rho_w);
     rec_suffix<Fr>(cx, wt.p, wt.p, H + 1, X, one, false);  // divide by v_X: q[i] = S[i + |X|]
-    Oracle o_w; o_w.p = wt.p + X; o_w.len = H + 1 - X; o_w.hiding = true;
+    LP o_w; o_w.p = wt.p + X; o_w.len = H + 1 - X; o_w.hiding = 1;
     blind(za_poly.p, rho_a);
     blind(zb_poly.p, rho_b);
-    Oracle o_za; o_za.p = za_poly.p; o_za.len = H + 1; o_za.hiding = true;
-    Oracle o_zb; o_zb.p = zb_poly.p; o_zb.len = H + 1; o_zb.hiding = true;
+    LP o_za; o_za.p = za_poly.p; o_za.len = H + 1; o_za.hiding = 1;
+    LP o_zb; o_zb.p = zb_poly.p; o_zb.len = H + 1; o_zb.hiding = 1;
     // mask polynomial: 3|H| rejection-sampled coefficients straight from the ChaCha stream
     DBuf<Fr> mask(cx, 3 * H);
     sample_mask(zk, mask.p, 3 * H);
@@ -663,11 +456,11 @@ struct MarlinIndex : IndexBase {
       Fr* pm = mask.p;
       ew(cx, 1, [=] __device__(size_t) { st_fr(pm, (ld_fr(pm + Hh) + ld_fr(pm + 2 * Hh)).neg()); });  // mask[0] -= sum_i mask[i|H|]
     }
-    Oracle o_mask; o_mask.p = mask.p; o_mask.len = 3 * H;
+    LP o_mask; o_mask.p = mask.p; o_mask.len = 3 * H;
     tm.end(t_r1);
     size_t t_c1 = tm.begin("Committing to first round polys");
-    std::vector<Oracle*> first = {&o_w, &o_za, &o_zb, &o_mask};
-    commit_round(first, zk);
+    std::vector<LP*> first = {&o_w, &o_za, &o_zb, &o_mask};
+    pc_commit(srs, msm, pc, first, zk);
     tm.end(t_c1);
     absorb_comms(fs, first);
     // verifier_first_round [reference verifier.rs:44-79]
@@ -748,13 +541,13 @@ struct MarlinIndex : IndexBase {
         if (i >= 1) st_fr(pg + i - 1, b0 + hi);  // g_1 = (X g_1) / X; coefficient 0 of X g_1 is zero
       });
     }
-    Oracle o_t; o_t.p = t_poly.p; o_t.len = H;
-    Oracle o_g1; o_g1.p = g1.p; o_g1.len = H - 1; o_g1.bounded = true; o_g1.bound = H - 2; o_g1.hiding = true;
-    Oracle o_h1; o_h1.p = h1.p; o_h1.len = 2 * H;
+    LP o_t; o_t.p = t_poly.p; o_t.len = H;
+    LP o_g1; o_g1.p = g1.p; o_g1.len = H - 1; o_g1.bound = H - 2; o_g1.hiding = 1;
+    LP o_h1; o_h1.p = h1.p; o_h1.len = 2 * H;
     tm.end(t_r2);
     size_t t_c2 = tm.begin("Committing to second round polys");
-    std::vector<Oracle*> second = {&o_t, &o_g1, &o_h1};
-    commit_round(second, zk);
+    std::vector<LP*> second = {&o_t, &o_g1, &o_h1};
+    pc_commit(srs, msm, pc, second, zk);
     tm.end(t_c2);
     absorb_comms(fs, second);
     Fr beta = sample_outside_h(fs);  // verifier_second_round
@@ -790,12 +583,12 @@ struct MarlinIndex : IndexBase {
       const Fr* pbf = bf.p; Fr* ph = h2.p;
       ew(cx, K, [=] __device__(size_t i) { st_fr(ph + i, ld_fr(pbf + Kk + i).neg()); });
     }
-    Oracle o_g2; o_g2.p = f_poly.p + 1; o_g2.len = K - 1; o_g2.bounded = true; o_g2.bound = K - 2;
-    Oracle o_h2; o_h2.p = h2.p; o_h2.len = K - 1;
+    LP o_g2; o_g2.p = f_poly.p + 1; o_g2.len = K - 1; o_g2.bound = K - 2;
+    LP o_h2; o_h2.p = h2.p; o_h2.len = K - 1;
     tm.end(t_r3);
     size_t t_c3 = tm.begin("Committing to third round polys");
-    std::vector<Oracle*> third = {&o_g2, &o_h2};
-    commit_round(third, zk);
+    std::vector<LP*> third = {&o_g2, &o_h2};
+    pc_commit(srs, msm, pc, third, zk);
     tm.end(t_c3);
     absorb_comms(fs, third);
     Fr gamma = field_rand<Fr>(fs);  // verifier_third_round
@@ -842,86 +635,29 @@ struct MarlinIndex : IndexBase {
 
     // ---- open_combinations [U ark-poly-commit marlin_pc / sonic_pc; SURVEY.md App. B] ---------------------
     size_t t_op = tm.begin("PC::open_combinations");
-    Fr xp[6];
-    xp[0] = one;
-    for (int i = 1; i < 6; i++) xp[i] = xp[i - 1] * xi;
-    const bool marlin = pc == B2M_PC_MARLIN_KZG10;
-    // challenge indices: Marlin PC burns two per degree-bounded polynomial, Sonic one per polynomial
-    const Fr ch_outer = marlin ? xp[2] : xp[1], ch_t = marlin ? xp[3] : xp[2], ch_zb = marlin ? xp[4] : xp[3];
-    const Fr ch_inner = marlin ? xp[2] : xp[1];
-    DBuf<Pt> w_out(cx, 2);
-    WitnessMsms<Fr, Fq> wit(cx);
-    typedef typename WitnessMsms<Fr, Fq>::Shifted Shifted;
-    HPoly r_beta;       // combined hiding randomness at beta
-    HPoly sr_beta;      // shifted randomness (Marlin PC): xi * shifted_rand(g_1)
-    {
-      // point beta: labels g_1, outer_sumcheck, t, z_b
-      DBuf<Fr> pbeta(cx, 3 * H), sbeta(cx, 3 * H);
-      LcTerms<Fr> lt;
-      lt.add(o_g1.p, o_g1.len, one);
-      lt.add(o_mask.p, o_mask.len, ch_outer);
-      lt.add(o_za.p, o_za.len, ch_outer * c_za);
-      lt.add(o_w.p, o_w.len, ch_outer * c_w);
-      lt.add(o_h1.p, o_h1.len, ch_outer * c_h1);
-      lt.add(o_t.p, o_t.len, ch_t);
-      lt.add(o_zb.p, o_zb.len, ch_zb);
-      lincomb(lt, 3 * H, pbeta.p);
-      rec_suffix<Fr>(cx, pbeta.p, sbeta.p, 3 * H, 1, beta, true);
-      hp_axpy(r_beta, one, o_g1.rand);
-      HPoly r_outer;
-      hp_axpy(r_outer, c_za, o_za.rand);
-      hp_axpy(r_outer, c_w, o_w.rand);
-      hp_axpy(r_beta, ch_outer, r_outer);
-      hp_axpy(r_beta, ch_zb, o_zb.rand);
-      HPoly hw = hp_is_zero(r_beta) ? HPoly() : hp_div_linear(r_beta, beta);  // hiding witness r / (X - beta)
-      std::vector<Shifted> shifted;
-      if (marlin) {
-        hp_axpy(sr_beta, xp[1], o_g1.shifted_rand);
-        if (!hp_is_zero(o_g1.shifted_rand)) hp_axpy(hw, xp[1], hp_div_linear(o_g1.shifted_rand, beta));
-        // shifted witness: xi * (g_1 / (X - beta)) against powers_of_g[D - (|H| - 2) ..]
-        shifted.push_back(Shifted{s_g1.p + 1, xp[1], o_g1.len - 1, shifted_off(o_g1.bound)});
-      }
-      wit.add_point(sbeta.p + 1, 3 * H - 1, shifted, hw, srs->gamma_slot(0), w_out.p);
-      // Both buffers (and pg, sg below) live until the MSMs have run: released here, they left the stream-ordered pool in a
-      // state where later allocations of this phase intermittently blocked in cudaMallocAsync for up to 0.3 s (H100, 2^20).
-      wit.keep_sc.push_back(std::move(sbeta));
-      wit.keep_sc.push_back(std::move(pbeta));
-    }
-    {
-      // point gamma: labels g_2, inner_sumcheck (nothing hiding)
-      DBuf<Fr> pg(cx, K), sg(cx, K);
-      LcTerms<Fr> lt;
-      lt.add(o_g2.p, o_g2.len, one);
-      lt.add(ipoly[2].p, K, ch_inner * ci_a);
-      lt.add(ipoly[3].p, K, ch_inner * ci_b);
-      lt.add(ipoly[4].p, K, ch_inner * ci_c);
-      lt.add(ipoly[0].p, K, ch_inner * ci_row);
-      lt.add(ipoly[1].p, K, ch_inner * ci_col);
-      lt.add(ipoly[5].p, K, ch_inner * ci_rc);
-      lt.add(o_h2.p, o_h2.len, ch_inner * ci_h2);
-      lincomb(lt, K, pg.p);
-      rec_suffix<Fr>(cx, pg.p, sg.p, K, 1, gamma, true);
-      std::vector<Shifted> shifted;
-      if (marlin) shifted.push_back(Shifted{s_g2.p + 1, xp[1], o_g2.len - 1, shifted_off(o_g2.bound)});
-      wit.add_point(sg.p + 1, K - 1, shifted, HPoly(), 0, w_out.p + 1);
-      wit.keep_sc.push_back(std::move(sg));
-      wit.keep_sc.push_back(std::move(pg));
-    }
-    wit.run(msm);
-    Pt w_pts[2];
-    w_out.download(w_pts, 2);
+    // g_1 and g_2 bring their quotients by (X - beta), (X - gamma) from the evaluations above
+    using Lc = OpenLc<Fr, Fq>;
+    std::vector<OpenPoint<Fr, Fq>> points(2);
+    points[0].z = beta;  // labels g_1, outer_sumcheck, t, z_b
+    points[0].lcs = {Lc{{{&o_g1, one}}, s_g1.p + 1}, Lc{{{&o_mask, one}, {&o_za, c_za}, {&o_w, c_w}, {&o_h1, c_h1}}}, Lc{{{&o_t, one}}},
+                     Lc{{{&o_zb, one}}}};
+    const LP* ip = index_polys;
+    points[1].z = gamma;  // labels g_2, inner_sumcheck
+    points[1].lcs = {Lc{{{&o_g2, one}}, s_g2.p + 1},
+                     Lc{{{&ip[2], ci_a}, {&ip[3], ci_b}, {&ip[4], ci_c}, {&ip[0], ci_row}, {&ip[1], ci_col}, {&ip[5], ci_rc}, {&o_h2, ci_h2}}}};
+    std::vector<Opening<Fr, Fq>> openings = pc_open(srs, msm, pc, xi, points);
     tm.end(t_op);
 
     // ---- Proof::new + CanonicalSerialize [reference data_structures.rs:100-126; SURVEY.md A.3] -----------
     proof.clear();
     put_u64(proof, 3);
-    std::vector<Oracle*>* rounds[3] = {&first, &second, &third};
+    std::vector<LP*>* rounds[3] = {&first, &second, &third};
     for (auto* rd : rounds) {
       put_u64(proof, rd->size());
       for (auto* o : *rd) {
         put_compressed(proof, o->comm);
-        if (marlin) {
-          if (o->bounded) { proof.push_back(1); put_compressed(proof, o->shifted_comm); }
+        if (pc == B2M_PC_MARLIN_KZG10) {
+          if (o->bound >= 0) { proof.push_back(1); put_compressed(proof, o->shifted_comm); }
           else proof.push_back(0);
         }
       }
@@ -931,21 +667,11 @@ struct MarlinIndex : IndexBase {
     put_u64(proof, 3);
     proof.push_back(0); proof.push_back(0); proof.push_back(0);  // three ProverMsg::EmptyMessage
     put_u64(proof, 2);
-    put_compressed(proof, w_pts[0]);
-    {
-      // random_v at beta: r(beta) (+ shifted_r(beta) for Marlin PC); Some iff the combined randomness is hiding
-      bool hiding = !hp_is_zero(r_beta);
-      if (hiding) {
-        Fr rv = hp_eval(r_beta, beta);
-        if (marlin) rv = rv + hp_eval(sr_beta, beta);
-        proof.push_back(1);
-        put_fr_canonical(proof, rv);
-      } else {
-        proof.push_back(0);
-      }
+    for (const auto& o : openings) {  // w || Option<random_v>
+      put_compressed(proof, o.w);
+      proof.push_back(o.hiding ? 1 : 0);
+      if (o.hiding) put_fr_canonical(proof, o.random_v);
     }
-    put_compressed(proof, w_pts[1]);
-    proof.push_back(0);  // gamma: no hiding polynomial is opened there
     proof.push_back(0);  // BatchLCProof.evals = None
     zk.commit_position();
     tm.end(t_all);
@@ -999,153 +725,54 @@ struct MarlinIndex : IndexBase {
 };
 
 // ---------------------------------------------------------------------------------------------------
-// Level 1: `PC::commit` over host polynomials [U ark-poly-commit marlin_pc / sonic_pc commit]
+// Level 1 over host polynomials: `PC::commit` and `PC::open_combinations` (b2m_pc_open: one coefficient-one combination per
+// polynomial, all at one point) [U ark-poly-commit marlin_pc / sonic_pc]
 // ---------------------------------------------------------------------------------------------------
+template <class Fr, class Fq>
+LabeledPoly<Fr, Fq> upload_poly(b2m_srs* srs, std::vector<DBuf<Fr>>& dev, size_t i, const uint64_t* coeffs, size_t len, int64_t bound) {
+  B2M_REQUIRE(len <= srs->n_g, B2M_ERR_DEGREE_TOO_LARGE, "polynomial %zu has %zu coefficients, the SRS %zu powers", i, len, srs->n_g);
+  dev.emplace_back(srs->ctx->cx, len ? len : 1);
+  if (len) dev.back().upload(reinterpret_cast<const Fr*>(coeffs), len);
+  LabeledPoly<Fr, Fq> q;
+  q.p = dev.back().p;
+  q.len = len;
+  q.bound = bound;
+  return q;
+}
+
 template <class Fr, class Fq>
 void pc_commit_impl(b2m_srs* srs, Msm<Fr, Fq>& msm, int pc, size_t n_polys, const uint64_t* const* coeffs, const size_t* n_coeffs,
                     const int64_t* degree_bounds, const int64_t* hiding_bounds, b2m_rng* rng, uint64_t* out_comm_xy,
                     uint64_t* out_shifted_xy, uint64_t* out_rand, uint64_t* out_shifted_rand, size_t rand_stride) {
-  using Pt = Affine<Fq>;
-  Ctx& cx = srs->ctx->cx;
   const size_t D = srs->n_g - 1;
-  const bool marlin = pc == B2M_PC_MARLIN_KZG10;
   bool any_hiding = false;
   for (size_t i = 0; i < n_polys; i++) any_hiding = any_hiding || hiding_bounds[i] >= 0;
   B2M_REQUIRE(!any_hiding || rng != nullptr, B2M_ERR_MISSING_RNG, "a hiding bound was requested but rng is null");
+  std::vector<DBuf<Fr>> dev;
+  std::vector<LabeledPoly<Fr, Fq>> polys;
+  for (size_t i = 0; i < n_polys; i++) {
+    const int64_t d = degree_bounds[i], hb = hiding_bounds[i];
+    polys.push_back(upload_poly<Fr, Fq>(srs, dev, i, coeffs[i], n_coeffs[i], d));
+    if (d >= 0)
+      B2M_REQUIRE((size_t)d <= D && n_coeffs[i] <= (size_t)d + 1, B2M_ERR_DEGREE_TOO_LARGE, "polynomial %zu exceeds its degree bound %lld", i, (long long)d);
+    if (hb >= 0)  // Randomness::rand: degree hiding_bound + 1
+      B2M_REQUIRE((size_t)hb + 2 <= rand_stride, B2M_ERR_INVALID_ARG, "rand_stride %zu < hiding bound %lld + 2", rand_stride, (long long)hb);
+    polys.back().hiding = hb;
+  }
+  std::vector<LabeledPoly<Fr, Fq>*> ptrs;
+  for (auto& q : polys) ptrs.push_back(&q);
   ZkSource<b2m_rng> zk(rng);
-  std::vector<DBuf<Fr>> polys, blind;
-  std::vector<MsmJob<Fr, Fq>> jobs;
-  DBuf<Pt> out(cx, 2 * n_polys);
-  B2M_CUDA(cudaMemsetAsync(out.p, 0, 2 * n_polys * sizeof(Pt), cx.stream));
+  pc_commit(srs, msm, pc, ptrs, zk);
   memset(out_rand, 0, n_polys * rand_stride * sizeof(Fr));
   if (out_shifted_rand) memset(out_shifted_rand, 0, n_polys * rand_stride * sizeof(Fr));
-  auto draw = [&](int64_t hb, uint64_t* dst) -> std::vector<Fr> {
-    std::vector<Fr> r;
-    if (hb < 0) return r;
-    B2M_REQUIRE((size_t)hb + 2 <= rand_stride, B2M_ERR_INVALID_ARG, "rand_stride %zu < hiding bound %lld + 2", rand_stride, (long long)hb);
-    for (int64_t k = 0; k < hb + 2; k++) r.push_back(field_rand<Fr>(zk));  // Randomness::rand: degree hiding_bound + 1
-    memcpy(dst, r.data(), r.size() * sizeof(Fr));
-    return r;
-  };
-  auto job = [&](const Fr* dev, size_t len, size_t off, const std::vector<Fr>& b, size_t gslot, Pt* dst) {
-    const Fr* s2 = nullptr;
-    if (!b.empty()) {
-      blind.emplace_back(cx, b.size());
-      blind.back().upload(b.data(), b.size());
-      s2 = blind.back().p;
-      for (size_t k = 1; k < b.size(); k++)
-        B2M_REQUIRE(srs->gamma_slot(srs->gamma_idx[gslot] + k) == gslot + k, B2M_ERR_INVALID_ARG, "gamma powers are not consecutive");
-    }
-    jobs.push_back(MsmJob<Fr, Fq>{dev, true, len, off, s2, b.size(), gslot, nullptr, 0, nullptr, dst});
-  };
   for (size_t i = 0; i < n_polys; i++) {
-    const size_t len = n_coeffs[i];
-    B2M_REQUIRE(len <= srs->n_g, B2M_ERR_DEGREE_TOO_LARGE, "polynomial %zu has %zu coefficients, the SRS %zu powers", i, len, srs->n_g);
-    polys.emplace_back(cx, len ? len : 1);
-    if (len) polys.back().upload(reinterpret_cast<const Fr*>(coeffs[i]), len);
-    const int64_t d = degree_bounds[i], hb = hiding_bounds[i];
-    if (d >= 0) {
-      B2M_REQUIRE((size_t)d <= D && len <= (size_t)d + 1, B2M_ERR_DEGREE_TOO_LARGE, "polynomial %zu exceeds its degree bound %lld", i, (long long)d);
-    }
-    if (marlin) {
-      job(polys.back().p, len, 0, draw(hb, out_rand + 4 * rand_stride * i), hb >= 0 ? srs->gamma_slot(0) : 0, out.p + 2 * i);
-      if (d >= 0)
-        job(polys.back().p, len, D - (size_t)d, draw(hb, out_shifted_rand + 4 * rand_stride * i), hb >= 0 ? srs->gamma_slot(0) : 0,
-            out.p + 2 * i + 1);
-    } else {
-      if (d >= 0) job(polys.back().p, len, D - (size_t)d, draw(hb, out_rand + 4 * rand_stride * i), hb >= 0 ? srs->gamma_slot(D - (size_t)d) : 0, out.p + 2 * i);
-      else job(polys.back().p, len, 0, draw(hb, out_rand + 4 * rand_stride * i), hb >= 0 ? srs->gamma_slot(0) : 0, out.p + 2 * i);
-    }
-  }
-  for (size_t at = 0; at < jobs.size(); at += MSM_MAX_BATCH)
-    msm.run_batch(jobs.data() + at, (int)std::min<size_t>(MSM_MAX_BATCH, jobs.size() - at));
-  std::vector<Pt> h(2 * n_polys);
-  out.download(h.data(), h.size());
-  for (size_t i = 0; i < n_polys; i++) {
-    memcpy(out_comm_xy + i * (2 * Fq::N / 2), &h[2 * i], sizeof(Pt));
-    if (out_shifted_xy) memcpy(out_shifted_xy + i * (2 * Fq::N / 2), &h[2 * i + 1], sizeof(Pt));
+    const LabeledPoly<Fr, Fq>& q = polys[i];
+    memcpy(out_comm_xy + i * (2 * Fq::N / 2), &q.comm, sizeof(q.comm));
+    if (out_shifted_xy) memcpy(out_shifted_xy + i * (2 * Fq::N / 2), &q.shifted_comm, sizeof(q.shifted_comm));
+    if (!q.rand.empty()) memcpy(out_rand + 4 * rand_stride * i, q.rand.data(), q.rand.size() * sizeof(Fr));
+    if (!q.shifted_rand.empty()) memcpy(out_shifted_rand + 4 * rand_stride * i, q.shifted_rand.data(), q.shifted_rand.size() * sizeof(Fr));
   }
   zk.commit_position();
-}
-
-// ---------------------------------------------------------------------------------------------------
-// Level 1: `PC::open_individual_opening_challenges` at one point [U ark-poly-commit marlin_pc / sonic_pc open]
-// ---------------------------------------------------------------------------------------------------
-template <class Fr>
-struct OpenItem {  // one labelled polynomial resident in HBM, with its commitment randomness
-  const Fr* dev;
-  size_t len;
-  int64_t bound;  // degree bound or -1
-  std::vector<Fr> rand, srand;  // blinding polynomials (trailing zeros stripped; empty = not hiding)
-};
-
-template <class Fr, class Fq>
-void pc_open_point_dev(b2m_srs* srs, Msm<Fr, Fq>& msm, int pc, const std::vector<OpenItem<Fr>>& items, int64_t max_degree_bound, const Fr& z,
-                       const Fr& xi, uint64_t* out_w_xy, int* out_has_random_v, uint64_t* out_random_v) {
-  using Pt = Affine<Fq>;
-  using M = MarlinIndex<Fr, Fq>;
-  typedef typename M::HPoly HPoly;
-  typedef typename WitnessMsms<Fr, Fq>::Shifted Shifted;
-  Ctx& cx = srs->ctx->cx;
-  const size_t D = srs->n_g - 1;
-  const bool marlin = pc == B2M_PC_MARLIN_KZG10;
-  const Fr one = Fr::one();
-  size_t max_len = 1;
-  for (auto& it : items) max_len = std::max(max_len, it.len);
-  std::vector<DBuf<Fr>> keep;
-  DBuf<Fr> comb(cx, max_len), tmp(cx, max_len);
-  comb.zero();
-  std::vector<Shifted> shifted;
-  HPoly r, sr, srw;
-  Fr ch = one;
-  bool enforce = false;
-  for (auto& it : items) {
-    const size_t len = it.len;
-    B2M_REQUIRE(len <= srs->n_g, B2M_ERR_DEGREE_TOO_LARGE, "a polynomial has %zu coefficients, the SRS %zu powers", len, srs->n_g);
-    // comb += ch * p_i
-    LcTerms<Fr> lt;
-    lt.add(comb.p, max_len, one);
-    lt.add(it.dev, len, ch);
-    lincomb_kernel<Fr><<<div_up(max_len, 256), 256, 0, cx.stream>>>(lt, max_len, tmp.p);
-    B2M_CHECK_LAUNCH();
-    cx.launches++;
-    std::swap(comb, tmp);
-    M::hp_axpy(r, ch, it.rand);
-    ch = ch * xi;
-    if (marlin && it.bound >= 0) {
-      B2M_REQUIRE(max_degree_bound >= it.bound && (size_t)max_degree_bound <= D, B2M_ERR_DEGREE_TOO_LARGE, "bad degree bounds");
-      enforce = true;
-      if (len > 1) {
-        // shifted witness ch1 * (p_i / (X - z)) against shifted_powers: powers_of_g[D - bound ..]
-        keep.emplace_back(cx, len);
-        rec_suffix<Fr>(cx, it.dev, keep.back().p, len, 1, z, true);
-        shifted.push_back(Shifted{keep.back().p + 1, ch, len - 1, D - (size_t)it.bound});
-      }
-      M::hp_axpy(sr, ch, it.srand);
-      if (!M::hp_is_zero(it.srand)) M::hp_axpy(srw, ch, M::hp_div_linear(it.srand, z));
-      ch = ch * xi;
-    }
-  }
-  // witness of the combination and its hiding part
-  DBuf<Fr> sfx(cx, max_len);
-  rec_suffix<Fr>(cx, comb.p, sfx.p, max_len, 1, z, true);
-  const bool hiding = !M::hp_is_zero(r);
-  HPoly hw = hiding ? M::hp_div_linear(r, z) : HPoly();
-  if (marlin && enforce) M::hp_axpy(hw, one, srw);
-  DBuf<Pt> w(cx, 1);
-  WitnessMsms<Fr, Fq> wit(cx);
-  wit.add_point(sfx.p + 1, max_len - 1, shifted, hw, hw.empty() ? 0 : srs->gamma_slot(0), w.p);
-  wit.run(msm);
-  Pt hwp;
-  w.download(&hwp, 1);
-  memcpy(out_w_xy, &hwp, sizeof(hwp));
-  *out_has_random_v = hiding ? 1 : 0;
-  Fr rv = Fr::zero();
-  if (hiding) {
-    rv = M::hp_eval(r, z);
-    if (marlin && enforce) rv = rv + M::hp_eval(sr, z);
-  }
-  memcpy(out_random_v, rv.l, sizeof(rv.l));
 }
 
 template <class Fr>
@@ -1162,91 +789,42 @@ static std::vector<Fr> host_rand_poly(const uint64_t* base, size_t rand_stride, 
 }
 
 template <class Fr, class Fq>
-void pc_open_impl(b2m_srs* srs, Ntt<Fr>& ntt, Msm<Fr, Fq>& msm, int pc, size_t n_polys, const uint64_t* const* coeffs,
-                  const size_t* n_coeffs, const int64_t* degree_bounds, const uint64_t* rands, const uint64_t* shifted_rands,
-                  size_t rand_stride, int64_t max_degree_bound, const uint64_t* point, const uint64_t* opening_challenge,
-                  uint64_t* out_w_xy, int* out_has_random_v, uint64_t* out_random_v) {
-  (void)ntt;
-  Ctx& cx = srs->ctx->cx;
-  Fr z, xi;
-  memcpy(z.l, point, sizeof(z.l));
-  memcpy(xi.l, opening_challenge, sizeof(xi.l));
-  std::vector<DBuf<Fr>> dev;
-  std::vector<OpenItem<Fr>> items;
-  for (size_t i = 0; i < n_polys; i++) {
-    const size_t len = n_coeffs[i];
-    B2M_REQUIRE(len <= srs->n_g, B2M_ERR_DEGREE_TOO_LARGE, "polynomial %zu has %zu coefficients, the SRS %zu powers", i, len, srs->n_g);
-    dev.emplace_back(cx, len ? len : 1);
-    if (len) dev.back().upload(reinterpret_cast<const Fr*>(coeffs[i]), len);
-    items.push_back(OpenItem<Fr>{dev.back().p, len, degree_bounds[i], host_rand_poly<Fr>(rands, rand_stride, i),
-                                 host_rand_poly<Fr>(shifted_rands, rand_stride, i)});
-  }
-  pc_open_point_dev<Fr, Fq>(srs, msm, pc, items, max_degree_bound, z, xi, out_w_xy, out_has_random_v, out_random_v);
-}
-
-// ---------------------------------------------------------------------------------------------------
-// Level 1: `PC::open_combinations` [U ark-poly-commit marlin_pc / sonic_pc open_combinations_individual_opening_challenges]
-// ---------------------------------------------------------------------------------------------------
-template <class Fr, class Fq>
 void pc_open_combinations_impl(b2m_srs* srs, Msm<Fr, Fq>& msm, int pc, int64_t max_degree_bound, size_t n_polys, const uint64_t* const* coeffs,
                                const size_t* n_coeffs, const int64_t* degree_bounds, const int* hiding, const uint64_t* rands,
                                const uint64_t* shifted_rands, size_t rand_stride, size_t n_lcs, const size_t* lc_term_off, const int64_t* lc_poly,
                                const uint64_t* lc_coeff, size_t n_queries, const size_t* query_lc, const size_t* query_point, size_t n_points,
                                const uint64_t* points, const uint64_t* opening_challenge, uint64_t* out_w_xy, int* out_has_random_v,
                                uint64_t* out_random_v) {
-  using M = MarlinIndex<Fr, Fq>;
-  Ctx& cx = srs->ctx->cx;
+  const size_t D = srs->n_g - 1;
   const bool marlin = pc == B2M_PC_MARLIN_KZG10;
+  const Fr one = Fr::one();
   Fr xi;
   memcpy(xi.l, opening_challenge, sizeof(xi.l));
-  const Fr one = Fr::one();
   std::vector<DBuf<Fr>> dev;
+  std::vector<LabeledPoly<Fr, Fq>> polys;
   for (size_t i = 0; i < n_polys; i++) {
-    const size_t len = n_coeffs[i];
-    B2M_REQUIRE(len <= srs->n_g, B2M_ERR_DEGREE_TOO_LARGE, "polynomial %zu has %zu coefficients, the SRS %zu powers", i, len, srs->n_g);
-    dev.emplace_back(cx, len ? len : 1);
-    if (len) dev.back().upload(reinterpret_cast<const Fr*>(coeffs[i]), len);
+    polys.push_back(upload_poly<Fr, Fq>(srs, dev, i, coeffs[i], n_coeffs[i], degree_bounds[i]));
+    if (hiding[i]) polys.back().rand = host_rand_poly<Fr>(rands, rand_stride, i);
+    if (hiding[i] && marlin && degree_bounds[i] >= 0) polys.back().shifted_rand = host_rand_poly<Fr>(shifted_rands, rand_stride, i);
   }
-  // the linear-combination polynomials, their randomness and degree bound
-  std::vector<DBuf<Fr>> lc_dev;
-  std::vector<OpenItem<Fr>> lcs;
+  std::vector<OpenLc<Fr, Fq>> lcs(n_lcs);
   for (size_t l = 0; l < n_lcs; l++) {
     const size_t t0 = lc_term_off[l], t1 = lc_term_off[l + 1];
-    size_t len = 1;
     for (size_t t = t0; t < t1; t++)
-      if (lc_poly[t] >= 0) {
-        B2M_REQUIRE((size_t)lc_poly[t] < n_polys, B2M_ERR_INVALID_ARG, "linear combination %zu names polynomial %lld of %zu", l, (long long)lc_poly[t], n_polys);
-        len = std::max(len, n_coeffs[lc_poly[t]]);
-      }
-    lc_dev.emplace_back(cx, len);
-    lc_dev.back().zero();
-    DBuf<Fr> tmp(cx, len);
-    OpenItem<Fr> item{nullptr, len, -1, {}, {}};
-    const size_t num_terms = t1 - t0;
+      B2M_REQUIRE(lc_poly[t] < 0 || (size_t)lc_poly[t] < n_polys, B2M_ERR_INVALID_ARG, "linear combination %zu names polynomial %lld of %zu", l,
+                  (long long)lc_poly[t], n_polys);
     for (size_t t = t0; t < t1; t++) {
       if (lc_poly[t] < 0) continue;  // LCTerm::One: affects the evaluation only
       const size_t i = (size_t)lc_poly[t];
       Fr c;
       memcpy(c.l, lc_coeff + 4 * t, sizeof(c.l));
-      if (degree_bounds[i] >= 0) {
-        B2M_REQUIRE(num_terms == 1 && c == one, B2M_ERR_INVALID_ARG,
-                    "linear combination %zu: a degree-bounded polynomial may only appear alone with coefficient one", l);
-        item.bound = degree_bounds[i];
-      }
-      LcTerms<Fr> lt;
-      lt.add(lc_dev.back().p, len, one);
-      lt.add(dev[i].p, n_coeffs[i], c);
-      lincomb_kernel<Fr><<<div_up(len, 256), 256, 0, cx.stream>>>(lt, len, tmp.p);
-      B2M_CHECK_LAUNCH();
-      cx.launches++;
-      std::swap(lc_dev.back(), tmp);
-      if (hiding[i]) M::hp_axpy(item.rand, c, host_rand_poly<Fr>(rands, rand_stride, i));
-      if (marlin && item.bound >= 0 && hiding[i]) M::hp_axpy(item.srand, c, host_rand_poly<Fr>(shifted_rands, rand_stride, i));
+      B2M_REQUIRE(degree_bounds[i] < 0 || (t1 - t0 == 1 && c == one), B2M_ERR_INVALID_ARG,
+                  "linear combination %zu: a degree-bounded polynomial may only appear alone with coefficient one", l);
+      lcs[l].terms.push_back({&polys[i], c});
     }
-    item.dev = lc_dev.back().p;
-    lcs.push_back(std::move(item));
   }
-  // one opening per point, the combinations queried there in label (= index) order
+  // the combinations queried at each point, in label (= index) order
+  std::vector<OpenPoint<Fr, Fq>> pts(n_points);
   for (size_t p = 0; p < n_points; p++) {
     std::vector<size_t> which;
     for (size_t q = 0; q < n_queries; q++)
@@ -1257,11 +835,19 @@ void pc_open_combinations_impl(b2m_srs* srs, Msm<Fr, Fq>& msm, int pc, int64_t m
     std::sort(which.begin(), which.end());
     which.erase(std::unique(which.begin(), which.end()), which.end());
     B2M_REQUIRE(!which.empty(), B2M_ERR_INVALID_ARG, "point %zu is not queried", p);
-    std::vector<OpenItem<Fr>> items;
-    for (size_t l : which) items.push_back(lcs[l]);
-    Fr z;
-    memcpy(z.l, points + 4 * p, sizeof(z.l));
-    pc_open_point_dev<Fr, Fq>(srs, msm, pc, items, max_degree_bound, z, xi, out_w_xy + p * (2 * Fq::N / 2), out_has_random_v + p, out_random_v + 4 * p);
+    memcpy(pts[p].z.l, points + 4 * p, sizeof(pts[p].z.l));
+    for (size_t l : which) {
+      const auto& t = lcs[l].terms;
+      if (marlin && t.size() == 1 && t[0].poly->bound >= 0)
+        B2M_REQUIRE(max_degree_bound >= t[0].poly->bound && (size_t)max_degree_bound <= D, B2M_ERR_DEGREE_TOO_LARGE, "bad degree bounds");
+      pts[p].lcs.push_back(lcs[l]);
+    }
+  }
+  std::vector<Opening<Fr, Fq>> res = pc_open(srs, msm, pc, xi, pts);
+  for (size_t p = 0; p < n_points; p++) {
+    memcpy(out_w_xy + p * (2 * Fq::N / 2), &res[p].w, sizeof(res[p].w));
+    out_has_random_v[p] = res[p].hiding ? 1 : 0;
+    memcpy(out_random_v + 4 * p, res[p].random_v.l, sizeof(res[p].random_v.l));
   }
 }
 

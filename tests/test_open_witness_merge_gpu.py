@@ -73,6 +73,7 @@ def test_prove_msm_count_and_pairs(gctx, curve_name, scheme, log_n):
     assert rep["msm_accumulate_kernel"]["launches"] == msms
     assert rep["msm_sort"]["launches"] == msms
     assert rep["msm_sort"]["units"] == pairs
+    assert rep["msm_reduce"]["launches"] == 4  # one batch per round's commitments, one for both opening points
     if log_n == 18:
         assert rep["msm_aff_level0"]["launches"] > 0  # the batched-affine levels are on at this size
 

@@ -461,7 +461,14 @@ def test_trim_and_open_combinations_level1(gctx, scheme):
             lc_idx = {lc.label: i for i, lc in enumerate(lcs)}
             glcs = [[(util.fr_to_mont_limbs(curve, [c])[0], None if t is None else label_idx[t]) for c, t in lc.terms] for lc in lcs]
             gqs = [(lc_idx[l], 0 if pl == "beta" else 1) for l, (pl, _) in qs]
-            got = m.open_combinations(ck, gp, rand, srand, glcs, gqs, util.fr_to_mont_limbs(curve, [z_beta, z_gamma]), util.fr_to_mont_limbs(curve, [xi])[0])
+            gctx.profile(True)
+            try:
+                got = m.open_combinations(ck, gp, rand, srand, glcs, gqs, util.fr_to_mont_limbs(curve, [z_beta, z_gamma]),
+                                          util.fr_to_mont_limbs(curve, [xi])[0])
+            finally:
+                rep = gctx.profile_report()
+                gctx.profile(False)
+            assert rep["msm_reduce"]["launches"] == 1  # the witness MSMs of both points in one batch
             assert len(got) == len(want) == 2
             for (gw, grv), (ow, orv) in zip(got, want):
                 assert util.points_from_limbs(curve, gw)[0] == ow
