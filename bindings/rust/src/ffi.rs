@@ -102,6 +102,19 @@ extern "C" {
     pub fn b2m_index_destroy(idx: *mut b2m_index);
     pub fn b2m_index_vk_bytes(idx: *const b2m_index, out: *mut u8, cap: usize, len: *mut usize) -> c_int;
     pub fn b2m_index_comms(idx: *const b2m_index, out_xy: *mut u64) -> c_int;
+    pub fn b2m_index_load(srs: *mut b2m_srs, pc_variant: c_int, num_constraints: usize, num_variables: usize,
+                          num_instance_variables: usize, num_non_zero: usize, a: *const b2m_matrix, b: *const b2m_matrix,
+                          c: *const b2m_matrix, vectors: *const *const u8, vector_lens: *const usize, index_comms_xy: *const u64,
+                          check_commitments: c_int, bad_vector: *mut usize, bad_index: *mut usize, bad_reason: *mut c_int,
+                          out: *mut *mut b2m_index) -> c_int;
+    pub fn b2m_index_sizes(idx: *const b2m_index, num_non_zero: *mut usize, domain_k: *mut usize, matrix_nnz: *mut usize) -> c_int;
+    pub fn b2m_index_export(idx: *mut b2m_index, vectors: *mut u8, row_ptrs: *const *mut u64, cols: *const *mut u64,
+                            coeffs: *const *mut u8) -> c_int;
+    pub fn b2m_fr_decode_ark(ctx: *mut b2m_ctx, curve: c_int, bytes: *const u8, n: usize, out_limbs: *mut u64, bad_index: *mut usize) -> c_int;
+    pub fn b2m_fr_to_canonical(ctx: *mut b2m_ctx, curve: c_int, limbs: *const u64, n: usize, out: *mut u8) -> c_int;
+    pub fn b2m_domain_ark(curve: c_int, log_size: c_uint, out: *mut u8) -> c_int;
+    pub fn b2m_ark_matrix_rows(bytes: *const u8, len: usize, n_rows: usize, entry_bytes: usize, row_ptr: *mut u64, end: *mut usize,
+                               bad_row: *mut usize, bad_reason: *mut c_int) -> c_int;
     pub fn b2m_prove(idx: *mut b2m_index, formatted_input: *const u64, n_input: usize, witness: *const u64, n_witness: usize,
                      zk_rng: *mut b2m_rng, proof: *mut u8, cap: usize, proof_len: *mut usize) -> c_int;
 

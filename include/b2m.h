@@ -156,6 +156,25 @@ int b2m_g2_decode_ark(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, i
 int b2m_g1_to_compressed(b2m_ctx* ctx, int curve, const uint64_t* points_xy, size_t n, uint8_t* out);
 int b2m_g2_to_compressed(int curve, const uint8_t* uncompressed, size_t n, uint8_t* out);
 
+/* Fr elements between the device and ark-serialize files (the index-key loader, marlin_b200/keyfile.py): canonical
+ * little-endian bytes (32 per element) to Montgomery limbs with `deserialize` semantics -- every value must be below r --
+ * and back.  Both run on the GPU, one thread per element, the decoder in chunks of 2^18 elements and the encoder in chunks
+ * of 2^20 elements, so device scratch stays bounded whatever n is.  An element >= r fails with
+ * B2M_ERR_SERIALIZATION and *bad_index receives the lowest such index (n on success; bad_index may be NULL). */
+int b2m_fr_decode_ark(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, uint64_t* out_limbs, size_t* bad_index);
+int b2m_fr_to_canonical(b2m_ctx* ctx, int curve, const uint64_t* limbs, size_t n, uint8_t* out);
+/* `Radix2EvaluationDomain::new(2^log_size)` as ark-serialize writes it [U ark-poly 0.3 domain/radix2]: size (u64),
+ * log_size_of_group (u32), then size_as_field_element, size_inv, group_gen, group_gen_inv, generator_inv as canonical Fr
+ * (12 + 5 * 32 = 172 bytes).  Host-side, no b2m_ctx needed. */
+int b2m_domain_ark(int curve, unsigned log_size, uint8_t* out);
+/* The row lengths of an ark-serialize `Vec<Vec<T>>` with fixed-size entries (a `Matrix<F>` has entry_bytes = 40: F then
+ * usize), after its outer u64 length: bytes[0 .. len) is the rest of the file.  row_ptr (n_rows + 1) receives the prefix sums
+ * of the row lengths and *end the byte length of the n_rows rows.  A row whose length field is cut short (bad_reason 1) or
+ * whose entries run past len (bad_reason 2) fails with B2M_ERR_SERIALIZATION, *bad_row = its index, *end = the offset of its
+ * length field.  Host-side, no b2m_ctx needed. */
+int b2m_ark_matrix_rows(const uint8_t* bytes, size_t len, size_t n_rows, size_t entry_bytes, uint64_t* row_ptr, size_t* end,
+                        size_t* bad_row, int* bad_reason);
+
 /* The caller's `zk_rng: &mut R` / `rng: Option<&mut dyn RngCore>` (reference src/lib.rs:154,125).  Two forms:
  *  - kind = B2M_RNG_CHACHA8/12/20, the fast path for the generators the reference's tests and benches use
  *    (`ark_std::test_rng()` = ChaCha12, `rand_chacha::ChaChaRng` = ChaCha20): the stream is described by its key and
@@ -272,6 +291,31 @@ void b2m_index_destroy(b2m_index* idx);
 int b2m_index_vk_bytes(const b2m_index* idx, uint8_t* out, size_t cap, size_t* len);
 /* Commitments to the index polynomials (affine x||y Montgomery, 6 points). */
 int b2m_index_comms(const b2m_index* idx, uint64_t* out_xy);
+
+/* An index from an `IndexProverKey` file instead of from `Marlin::index`: the matrices (as b2m_index_create takes them; the
+ * index keeps them in this row form for b2m_index_export), num_non_zero = |joint matrix| (index_info.num_non_zero) and the
+ * twelve index vectors as canonical little-endian Fr bytes in HOST memory (e.g. a memory-mapped file): vectors[0..6) the
+ * coefficients of row, col, a_val, b_val, c_val, row_col (vector_lens[i] <= |K|, zero-padded to |K|), vectors[6..12) their
+ * evaluations on K in the same order (vector_lens[i] == |K|).  index_comms_xy: the six commitments (affine x||y Montgomery).
+ * The vectors are decoded on the GPU straight into the index's device buffers; no arithmetization and no commitment MSM
+ * runs.  Checked on the GPU: every element is below r, and the NTT over K of each zero-padded coefficient vector equals its
+ * evaluations.  check_commitments != 0 also recomputes the six commitments (`PC::commit`, rng = None) and compares them.
+ * A failed check returns B2M_ERR_SERIALIZATION with *bad_vector (0..11, or 0..5 for a commitment), *bad_index (the lowest
+ * bad element) and *bad_reason (1 not below r, 2 evaluations differ from the NTT of the coefficients, 3 commitment
+ * differs); the pointers may be NULL.  Dimension errors are those of b2m_index_create, and num_non_zero must lie between
+ * the entry count of the largest matrix and the sum of the three. */
+int b2m_index_load(b2m_srs* srs, int pc_variant, size_t num_constraints, size_t num_variables, size_t num_instance_variables,
+                   size_t num_non_zero, const b2m_matrix* a, const b2m_matrix* b, const b2m_matrix* c,
+                   const uint8_t* const* vectors, const size_t* vector_lens, const uint64_t* index_comms_xy,
+                   int check_commitments, size_t* bad_vector, size_t* bad_index, int* bad_reason, b2m_index** out);
+/* num_non_zero, |K| and the entries of A, B, C (matrix_nnz[3]) of an index: the buffer sizes b2m_index_export needs. */
+int b2m_index_sizes(const b2m_index* idx, size_t* num_non_zero, size_t* domain_k, size_t* matrix_nnz);
+/* The index as an `IndexProverKey` file holds it, converted on the GPU: vectors (12 * |K| * 32 bytes) receives the
+ * coefficient vectors (zero-padded to |K|) then the evaluation vectors, in b2m_index_load's order, as canonical Fr bytes;
+ * row_ptrs[m] (num_constraints + 1), cols[m] (matrix_nnz[m]) and coeffs[m] (32 * matrix_nnz[m] canonical bytes) receive
+ * matrix m = A, B, C in the row form the index was given.  Any output pointer may be NULL to skip it. */
+int b2m_index_export(b2m_index* idx, uint8_t* vectors, uint64_t* const* row_ptrs, uint64_t* const* cols,
+                     uint8_t* const* coeffs);
 
 
 /* Replaces `Marlin::prove` (reference src/lib.rs:151-311).  formatted_input: the instance

@@ -86,6 +86,10 @@ def lib():
         L.b2m_g2_decode_ark.argtypes = [vp, ci, vp, sz, ci, vp, P(sz), P(ci)]
         L.b2m_g1_to_compressed.argtypes = [vp, ci, vp, sz, vp]
         L.b2m_g2_to_compressed.argtypes = [ci, vp, sz, vp]
+        L.b2m_fr_decode_ark.argtypes = [vp, ci, vp, sz, vp, P(sz)]
+        L.b2m_fr_to_canonical.argtypes = [vp, ci, vp, sz, vp]
+        L.b2m_domain_ark.argtypes = [ci, ctypes.c_uint, vp]
+        L.b2m_ark_matrix_rows.argtypes = [vp, sz, sz, sz, vp, P(sz), P(sz), P(ci)]
         L.b2m_pc_commit.argtypes = [vp, ci, sz, vp, vp, vp, vp, P(Rng), vp, vp, vp, vp, sz]
         L.b2m_pc_open.argtypes = [vp, ci, sz, vp, vp, vp, vp, vp, sz, ctypes.c_int64, vp, vp, vp, P(ci), vp]
         L.b2m_trim.argtypes = [vp, ci, sz, sz, vp, sz, P(vp)]
@@ -102,6 +106,9 @@ def lib():
             L.b2m_index_destroy.restype = None
             L.b2m_index_vk_bytes.argtypes = [vp, vp, sz, P(sz)]
             L.b2m_index_comms.argtypes = [vp, vp]
+            L.b2m_index_load.argtypes = [vp, ci, sz, sz, sz, sz, P(Matrix), P(Matrix), P(Matrix), vp, vp, vp, ci, P(sz), P(sz), P(ci), P(vp)]
+            L.b2m_index_sizes.argtypes = [vp, P(sz), P(sz), vp]
+            L.b2m_index_export.argtypes = [vp, vp, vp, vp, vp]
             L.b2m_index_stage.argtypes = [vp, vp, sz, vp, sz]
             L.b2m_prove.argtypes = [vp, vp, sz, vp, sz, P(Rng), vp, sz, P(sz)]
             L.b2m_prove_timings.argtypes = [vp, ctypes.c_char_p, sz]

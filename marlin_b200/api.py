@@ -10,10 +10,12 @@ batch on the host); `Marlin.verify` is a batch of one.
 import ctypes
 import json
 import os
+import struct
+import types
 
 import numpy as np
 
-from . import _lib, fields
+from . import _lib, fields, srsfile
 
 PC_IDS = {"marlin_kzg10": _lib.PC_MARLIN_KZG10, "sonic_kzg10": _lib.PC_SONIC_KZG10}
 
@@ -191,9 +193,13 @@ class UniversalSRS:
 
 
 class IndexProverKey:
+    """`IndexProverKey` on the device (b2m_index).  `r1cs` supplies num_constraints, num_variables and num_instance."""
+
     def __init__(self, srs, handle, r1cs, pc):
         self.srs, self.handle, self.pc = srs, handle, pc
         self.num_constraints, self.num_variables = r1cs.num_constraints, r1cs.num_variables
+        self.num_instance = r1cs.num_instance
+        self.file_g2 = None  # (h, beta_h, {D - d: neg power}) as uncompressed bytes, when loaded from a key file
         L = _lib.lib()
         n = ctypes.c_size_t(0)
         _lib.check(L.b2m_index_vk_bytes(handle, None, 0, ctypes.byref(n)))
@@ -208,6 +214,82 @@ class IndexProverKey:
         buf = ctypes.create_string_buffer(4096)
         _lib.check(_lib.lib().b2m_prove_timings(self.handle, buf, 4096))
         return json.loads(buf.value.decode() or "{}")
+
+    def info(self):
+        """`IndexInfo`: (num_variables, num_constraints, num_non_zero, num_instance_variables)"""
+        nv, nc, nnz = struct.unpack_from("<QQQ", self.vk_bytes, 0)
+        return nv, nc, nnz, self.num_instance
+
+    def _vk_fields(self, compressed):
+        """`IndexVerifierKey` of this index as marlin_b200.keyfile writes it: the verifier key `PC::trim` makes for the
+        enforced bounds {|H| - 2, |K| - 2} (sorted, deduplicated), supported_degree = the index's max degree, max_degree = D."""
+        from . import srsfile
+        srs, cid = self.srs, self.srs.curve_id
+        nv, nc, nnz, ni = self.info()
+        D = srs.max_degree
+        bounds = index_degree_bounds(nc, nnz)
+        h, beta_h, neg = self.file_g2 or g2_half(srs, bounds)
+        powers = np.ascontiguousarray(srs.powers_limbs)
+        g1 = lambda limbs: g1_to_bytes(srs.ctx, cid, limbs, compressed)
+        g2 = lambda unc: g2_to_bytes(cid, unc, compressed)
+        if self.pc == _lib.PC_MARLIN_KZG10:
+            bound_points = g1(np.stack([powers[D - d] for d in bounds]))
+        else:
+            missing = [d for d in bounds if D - d not in neg]
+            if missing:
+                raise ValueError(f"the SRS holds no neg_powers_of_h for the degree bounds {missing}")
+            bound_points = g2(np.frombuffer(b"".join(neg[D - d] for d in bounds), dtype=np.uint8))
+        g1b, g2b = srsfile.point_sizes(cid, compressed)
+        return {"info": (nv, nc, nnz, ni), "comms": g1(self.index_comms).reshape(6, g1b), "g": g1(powers[:1]),
+                "gamma_g": g1(srs.gamma_limbs[[list(srs.gamma_indices).index(0)]]), "h": g2(np.frombuffer(h, dtype=np.uint8)),
+                "beta_h": g2(np.frombuffer(beta_h, dtype=np.uint8)), "bounds": bounds, "bound_points": bound_points.reshape(len(bounds), -1),
+                "supported_degree": max_degree(nc, nv, nnz), "max_degree": D}
+
+    def save_verifier_key(self, path, compressed=True):
+        """Write the `IndexVerifierKey` `Marlin::index` returns for this index as a raw ark-serialize file
+        (marlin_b200/keyfile.py).  The G2 half comes from the SRS trapdoor or its source file, as `Marlin.verifier_key` takes it."""
+        from . import keyfile
+        keyfile.write_verifier_key(path, self.pc, self._vk_fields(compressed))
+
+    def save(self, path, compressed=True):
+        """Write the `IndexProverKey` `Marlin::index` returns for this index as a raw ark-serialize file
+        (marlin_b200/keyfile.py): the verifier key, empty commitment randomness, the matrices as the index received them,
+        the six index polynomials (trailing zero coefficients stripped) with their evaluations on K, and the committer key
+        `PC::trim` makes from the SRS.  Field elements are converted to canonical form on the GPU."""
+        from . import keyfile
+        L = _lib.lib()
+        srs, cid = self.srs, self.srs.curve_id
+        vk = self._vk_fields(compressed)
+        nv, nc, nnz, ni = vk["info"]
+        nnz_c, K = ctypes.c_size_t(0), ctypes.c_size_t(0)
+        mnnz = np.zeros(3, dtype=np.uint64)
+        _lib.check(L.b2m_index_sizes(self.handle, ctypes.byref(nnz_c), ctypes.byref(K), _lib.ptr(mnnz)))
+        K = K.value
+        vectors = np.zeros((12, K, keyfile.FR_BYTES), dtype=np.uint8)
+        row_ptrs = [np.zeros(nc + 1, dtype=np.uint64) for _ in range(3)]
+        cols = [np.zeros(max(int(n), 1), dtype=np.uint64) for n in mnnz]
+        coeffs = [np.zeros((max(int(n), 1), keyfile.FR_BYTES), dtype=np.uint8) for n in mnnz]
+        arr = lambda xs: (ctypes.c_void_p * 3)(*[x.ctypes.data for x in xs])
+        _lib.check(L.b2m_index_export(self.handle, _lib.ptr(vectors), arr(row_ptrs), arr(cols), arr(coeffs)))
+        mats = [(row_ptrs[m], cols[m][:int(mnnz[m])], coeffs[m][:int(mnnz[m])]) for m in range(3)]
+        dom = domain_bytes(cid, K)
+        index = {"info": vk["info"], "matrices": mats, "coeffs": list(vectors[:6]), "evals": list(vectors[6:]), "domains": [dom] * 6}
+        D = srs.max_degree
+        bounds = vk["bounds"]
+        md = vk["supported_degree"]
+        powers = np.ascontiguousarray(srs.powers_limbs)
+        g1 = lambda limbs: g1_to_bytes(srs.ctx, cid, limbs, compressed)
+        gamma = lambda idx: g1(srs_gamma_powers(srs, idx))
+        ck = {"powers": g1(powers[:md + 1]), "shifted": g1(powers[D - bounds[-1]:]), "gamma": gamma([0, 1, 2]), "bounds": bounds,
+              "max_degree": D}
+        if self.pc == _lib.PC_SONIC_KZG10:
+            ck["shifted_gamma"] = {d: gamma([D - d + i for i in range(3) if D - d + i < D + 2]) for d in bounds}
+        g1b, _ = srsfile.point_sizes(cid, compressed)
+        for k in ("powers", "shifted", "gamma"):
+            ck[k] = ck[k].reshape(-1, g1b)
+        if "shifted_gamma" in ck:
+            ck["shifted_gamma"] = {d: v.reshape(-1, g1b) for d, v in ck["shifted_gamma"].items()}
+        keyfile.write_prover_key(path, self.pc, vk, index, ck)
 
     def close(self):
         if self.handle:
@@ -231,6 +313,75 @@ class VerifierKey:
         if self.handle:
             _lib.lib().b2m_vk_destroy(self.handle)
             self.handle = None
+
+
+def _p2(n):
+    s = 1
+    while s < n:
+        s *= 2
+    return s
+
+
+def index_degree_bounds(num_constraints, num_non_zero):
+    """The bounds `Marlin::index` enforces, {|H| - 2, |K| - 2} sorted and deduplicated [reference src/ahp/mod.rs:96-106]"""
+    return sorted({_p2(num_constraints) - 2, _p2(num_non_zero) - 2})
+
+
+def g2_half(srs, bounds):
+    """h, beta h and {D - d: beta^-(D - d) h} per bound d (uncompressed bytes) of an SRS: from its trapdoor, or from the file
+    it was loaded from."""
+    from . import srsfile
+    cid = srs.curve_id
+    if srs.trapdoor is not None:
+        return srsfile.g2_setup(cid, fields.FR_MODULUS[cid], srs.trapdoor[0], srs.max_degree, bounds)
+    if srs.g2 is not None:
+        return srs.g2
+    raise ValueError("this SRS has no G2 half (neither a trapdoor nor a source file)")
+
+
+def g1_to_bytes(ctx, cid, limbs, compressed):
+    """affine Montgomery limbs -> ark-serialize G1 bytes (GPU), flat uint8"""
+    limbs = np.ascontiguousarray(limbs, dtype=np.uint64).reshape(-1, 2 * _lib.LIMBS[cid][1])
+    g1, _ = srsfile.point_sizes(cid, compressed)
+    out = np.zeros(len(limbs) * g1, dtype=np.uint8)
+    conv = _lib.lib().b2m_g1_to_compressed if compressed else _lib.lib().b2m_g1_to_uncompressed
+    _lib.check(conv(ctx.handle, cid, _lib.ptr(limbs), len(limbs), _lib.ptr(out)))
+    return out
+
+
+def g2_to_bytes(cid, unc, compressed):
+    """uncompressed G2 bytes -> the chosen form, flat uint8"""
+    unc = np.ascontiguousarray(unc, dtype=np.uint8).reshape(-1)
+    if not compressed:
+        return unc
+    _, g2 = srsfile.point_sizes(cid, True)
+    n = unc.size // (2 * g2)
+    out = np.zeros(n * g2, dtype=np.uint8)
+    _lib.check(_lib.lib().b2m_g2_to_compressed(cid, _lib.ptr(unc), n, _lib.ptr(out)))
+    return out
+
+
+def srs_gamma_powers(srs, idx):
+    """powers_of_gamma_g at the given exponents, affine limbs: from the whole source file when there is one, else from the
+    powers on the device"""
+    if srs.ark is not None:
+        keys, limbs = srs.ark["gamma_keys"], srs.ark["gamma_limbs"]
+    else:
+        keys, limbs = np.asarray(srs.gamma_indices, dtype=np.uint64), np.asarray(srs.gamma_limbs)
+    out = []
+    for i in idx:
+        hit = np.flatnonzero(keys == np.uint64(i))
+        if not len(hit):
+            raise ValueError(f"the SRS holds no powers_of_gamma_g[{i}]")
+        out.append(limbs[int(hit[0])])
+    return np.stack(out)
+
+
+def domain_bytes(cid, size):
+    """`Radix2EvaluationDomain::new(size)` as ark-serialize writes it (b2m_domain_ark)"""
+    out = np.zeros(172, dtype=np.uint8)
+    _lib.check(_lib.lib().b2m_domain_ark(cid, size.bit_length() - 1, _lib.ptr(out)))
+    return out.tobytes()
 
 
 def max_degree(num_constraints, num_variables, num_non_zero):
@@ -486,6 +637,192 @@ class Marlin:
                                       ctypes.byref(a), ctypes.byref(b), ctypes.byref(c), ctypes.byref(h)))
         return IndexProverKey(srs, h, r1cs, self.pc)
 
+    # -- index key files (marlin_b200/keyfile.py) --------------------------------------------------------
+    def _decode_g1(self, pts, field, compressed, names=int):
+        """ark-serialize G1 bytes (n, size) -> affine limbs, validated on the GPU; an invalid point raises naming field[index]"""
+        L = _lib.lib()
+        pts = np.ascontiguousarray(pts, dtype=np.uint8)
+        n = len(pts)
+        out = np.zeros((n, 2 * _lib.LIMBS[self.curve_id][1]), dtype=np.uint64)
+        if n == 0:
+            return out
+        bi, br = ctypes.c_size_t(0), ctypes.c_int(0)
+        rc = L.b2m_g1_decode_ark(self.ctx.handle, self.curve_id, _lib.ptr(pts.reshape(-1)), n, int(compressed), _lib.ptr(out), ctypes.byref(bi),
+                                 ctypes.byref(br))
+        if rc == _lib.ERR_SERIALIZATION:
+            raise _lib.B2MError(rc, f"{field}[{names(bi.value)}]: {_lib.POINT_REASONS.get(br.value, 'invalid point')}")
+        _lib.check(rc)
+        return out
+
+    def _decode_g2(self, pts, field, compressed, names=int):
+        """ark-serialize G2 bytes (n, size) -> uncompressed canonical bytes (n, 4 sizeof(Fq)), validated on the GPU"""
+        from . import srsfile
+        L = _lib.lib()
+        pts = np.ascontiguousarray(pts, dtype=np.uint8)
+        n = len(pts)
+        out = np.zeros((n, 4 * srsfile.fq_bytes(self.curve_id)), dtype=np.uint8)
+        if n == 0:
+            return out
+        bi, br = ctypes.c_size_t(0), ctypes.c_int(0)
+        rc = L.b2m_g2_decode_ark(self.ctx.handle, self.curve_id, _lib.ptr(pts.reshape(-1)), n, int(compressed), _lib.ptr(out), ctypes.byref(bi),
+                                 ctypes.byref(br))
+        if rc == _lib.ERR_SERIALIZATION:
+            at = "" if names is None else f"[{names(bi.value)}]"
+            raise _lib.B2MError(rc, f"{field}{at}: {_lib.POINT_REASONS.get(br.value, 'invalid point')}")
+        _lib.check(rc)
+        return out
+
+    def _decode_vk(self, vk, compressed):
+        """Every point of a parsed `IndexVerifierKey`, decoded and validated on the GPU"""
+        f = "index_vk.verifier_key"
+        out = {"comms": self._decode_g1(vk["comms"], "index_vk.index_comms", compressed),
+               "g": self._decode_g1(vk["g"].reshape(1, -1), f + ".g", compressed)[0],
+               "gamma_g": self._decode_g1(vk["gamma_g"].reshape(1, -1), f + ".gamma_g", compressed)[0]}
+        out["h"] = self._decode_g2(vk["h"].reshape(1, -1), f + ".h", compressed, None)[0]
+        out["beta_h"] = self._decode_g2(vk["beta_h"].reshape(1, -1), f + ".beta_h", compressed, None)[0]
+        keys = vk["bounds"]
+        if self.pc == _lib.PC_MARLIN_KZG10:
+            out["bound_points"] = self._decode_g1(vk["bound_points"], f + ".degree_bounds_and_shift_powers", compressed)
+        else:
+            out["bound_points"] = self._decode_g2(vk["bound_points"], f + ".degree_bounds_and_neg_powers_of_h", compressed)
+        return out
+
+    def _make_vk(self, vk, pts):
+        nv, nc, nnz, _ = vk["info"]
+        L = _lib.lib()
+        b = np.asarray(vk["bounds"], dtype=np.uint64)
+        handle = ctypes.c_void_p()
+        _lib.check(L.b2m_vk_create(self.ctx.handle, self.curve_id, self.pc, nc, nv, nnz, _lib.ptr(np.ascontiguousarray(pts["comms"])),
+                                   _lib.ptr(np.ascontiguousarray(pts["g"])), _lib.ptr(np.ascontiguousarray(pts["gamma_g"])),
+                                   _lib.ptr(np.ascontiguousarray(pts["h"])), _lib.ptr(np.ascontiguousarray(pts["beta_h"])), len(b),
+                                   _lib.ptr(b) if len(b) else None, _lib.ptr(np.ascontiguousarray(pts["bound_points"])) if len(b) else None,
+                                   ctypes.byref(handle)))
+        return VerifierKey(self.ctx, handle, self.curve_id, self.pc)
+
+    def load_verifier_key(self, path, compressed=True):
+        """A `VerifierKey` from a raw arkworks `IndexVerifierKey` file alone (`serialize` when compressed, else
+        `serialize_uncompressed`; marlin_b200/keyfile.py): no SRS and no index are needed.  Every point is decoded and validated
+        on the GPU; an invalid one raises B2MError (B2M_ERR_SERIALIZATION) naming its field and index."""
+        from . import keyfile
+        vk = keyfile.read_verifier_key(path, self.curve_id, self.pc, compressed)
+        return self._make_vk(vk, self._decode_vk(vk, compressed))
+
+    def load_index(self, srs, path, compressed=True, check_commitments=False):
+        """An `IndexProverKey` from a raw arkworks key file, on `srs`, without re-indexing: no arithmetization and no commitment
+        MSM run.  Every point is decoded and validated on the GPU (b2m_g1_decode_ark / b2m_g2_decode_ark), every field element
+        is checked to be below r on the GPU, and the NTT over K of each index polynomial must equal its evaluations
+        (b2m_index_load).  The committer key and the verifier key's G1 part must be those `PC::trim` makes from `srs` for the
+        bounds {|H| - 2, |K| - 2}.  check_commitments=True also recomputes the six index commitments.  A failure raises
+        B2MError (B2M_ERR_SERIALIZATION) or ValueError naming the field and the first bad index, e.g.
+        `index.joint_arith.evals_on_K.val_b[70001]: not below the field modulus`."""
+        from . import keyfile
+        L = _lib.lib()
+        cid, marlin = self.curve_id, self.pc == _lib.PC_MARLIN_KZG10
+        d = keyfile.read_prover_key(path, cid, self.pc, compressed)
+        vk, idx, ck = d["vk"], d["index"], d["ck"]
+        nv, nc, nnz, ni = vk["info"]
+        pts = self._decode_vk(vk, compressed)
+        ckn = "committer_key." + ("powers" if marlin else "powers_of_g")
+        shn = "committer_key." + ("shifted_powers" if marlin else "shifted_powers_of_g")
+        ck_powers = self._decode_g1(ck["powers"], ckn, compressed)
+        ck_shifted = self._decode_g1(ck["shifted"], shn, compressed) if ck["shifted"] is not None else None
+        ck_gamma = self._decode_g1(ck["gamma"], "committer_key.powers_of_gamma_g", compressed)
+        ck_sgamma = {}
+        for k, v in (ck.get("shifted_gamma") or {}).items():
+            ck_sgamma[k] = self._decode_g1(v, f"committer_key.shifted_powers_of_gamma_g[{k}]", compressed)
+
+        # the committer key and the verifier key's G1 part against the SRS they are loaded onto
+        D = srs.max_degree
+        bounds = index_degree_bounds(nc, nnz)
+        md = max_degree(nc, nv, nnz)
+        powers = np.asarray(srs.powers_limbs)
+
+        def same(field, got, want, offset=0):
+            got, want = np.asarray(got).reshape(len(got), -1), np.asarray(want).reshape(len(want), -1)
+            if len(got) != len(want):
+                raise ValueError(f"{path}: {field}: {len(got)} points, the SRS gives {len(want)}")
+            diff = np.flatnonzero(np.any(got != want, axis=1))
+            if len(diff):
+                raise ValueError(f"{path}: {field}[{int(diff[0]) + offset}]: differs from the SRS")
+
+        def equal(field, got, want):
+            if got != want:
+                raise ValueError(f"{path}: {field} is {got}, expected {want}")
+        equal("committer_key.max_degree", ck["max_degree"], D)
+        equal("committer_key.enforced_degree_bounds", ck["bounds"], bounds)
+        equal("index_vk.verifier_key.max_degree", vk["max_degree"], D)
+        equal("index_vk.verifier_key.supported_degree", vk["supported_degree"], md)
+        equal("index_vk.verifier_key degree bounds", [int(b) for b in vk["bounds"]], bounds)
+        if md > D:
+            raise ValueError(f"{path}: the index needs max degree {md}, the SRS has {D}")
+        same(ckn, ck_powers, powers[:md + 1])
+        if ck_shifted is None:
+            raise ValueError(f"{path}: {shn} is None, the index enforces degree bounds {bounds}")
+        same(shn, ck_shifted, powers[D - bounds[-1]:])
+        same("committer_key.powers_of_gamma_g", ck_gamma, srs_gamma_powers(srs, [0, 1, 2]))
+        if not marlin:
+            equal("committer_key.shifted_powers_of_gamma_g keys", sorted(ck_sgamma), bounds)
+            for k in bounds:
+                same(f"committer_key.shifted_powers_of_gamma_g[{k}]", ck_sgamma[k], srs_gamma_powers(srs, [D - k + i for i in range(3) if D - k + i < D + 2]))
+        same("index_vk.verifier_key.g", pts["g"].reshape(1, -1), powers[:1])
+        same("index_vk.verifier_key.gamma_g", pts["gamma_g"].reshape(1, -1), srs_gamma_powers(srs, [0]))
+        if marlin:
+            same("index_vk.verifier_key.degree_bounds_and_shift_powers", pts["bound_points"], np.stack([powers[D - b] for b in bounds]))
+
+        # the index: sizes and domains, matrices (coefficients decoded on the GPU), then the twelve vectors
+        K = _p2(nnz)
+        dom = domain_bytes(cid, K)
+        for i, name in enumerate(keyfile.POLY_LABELS):
+            ename = keyfile.EVAL_NAMES[keyfile.EVAL_OF_POLY[i]]
+            if len(idx["evals"][i]) != K:
+                raise ValueError(f"{path}: index.joint_arith.evals_on_K.{ename}.evals has {len(idx['evals'][i])} elements, |K| = {K}")
+            if idx["domains"][i] != dom:
+                raise ValueError(f"{path}: index.joint_arith.evals_on_K.{ename}.domain is not the domain of size {K}")
+            if len(idx["coeffs"][i]) > K:
+                raise ValueError(f"{path}: index.joint_arith.{name}.polynomial has {len(idx['coeffs'][i])} coefficients, |K| = {K}")
+        mats, keep = [], []
+        for m, (row_ptr, col, coeff) in zip(keyfile.MATRICES, idx["matrices"]):
+            if len(row_ptr) != nc + 1:
+                raise ValueError(f"{path}: index.{m} has {len(row_ptr) - 1} rows, num_constraints is {nc}")
+            ne = len(col)
+            limbs = np.zeros((max(ne, 1), 4), dtype=np.uint64)
+            bi = ctypes.c_size_t(0)
+            rc = L.b2m_fr_decode_ark(self.ctx.handle, cid, _lib.ptr(np.ascontiguousarray(coeff)), ne, _lib.ptr(limbs), ctypes.byref(bi))
+            if rc == _lib.ERR_SERIALIZATION:
+                r = int(np.searchsorted(row_ptr, np.uint64(bi.value), side="right")) - 1
+                raise _lib.B2MError(rc, f"index.{m}[{r}][{bi.value - int(row_ptr[r])}].0: not below the field modulus")
+            _lib.check(rc)
+            col = np.ascontiguousarray(col, dtype=np.uint64) if ne else np.zeros(1, dtype=np.uint64)
+            row_ptr = np.ascontiguousarray(row_ptr, dtype=np.uint64)
+            keep += [row_ptr, col, limbs]
+            mt = _lib.Matrix()
+            mt.row_ptr, mt.col, mt.coeff = row_ptr.ctypes.data, col.ctypes.data, limbs.ctypes.data
+            mats.append(mt)
+        vecs = [np.ascontiguousarray(v) for v in idx["coeffs"] + idx["evals"]]
+        vptr = (ctypes.c_void_p * 12)(*[v.ctypes.data if len(v) else None for v in vecs])
+        vlen = (ctypes.c_size_t * 12)(*[len(v) for v in vecs])
+        h = ctypes.c_void_p()
+        bv, bi, br = ctypes.c_size_t(0), ctypes.c_size_t(0), ctypes.c_int(0)
+        rc = L.b2m_index_load(srs.handle, self.pc, nc, nv, ni, nnz, ctypes.byref(mats[0]), ctypes.byref(mats[1]), ctypes.byref(mats[2]), vptr, vlen,
+                              _lib.ptr(np.ascontiguousarray(pts["comms"])), int(check_commitments), ctypes.byref(bv), ctypes.byref(bi),
+                              ctypes.byref(br), ctypes.byref(h))
+        if rc == _lib.ERR_SERIALIZATION and br.value:
+            v, i = bv.value, bi.value
+            label = keyfile.POLY_LABELS[v % 6]
+            ev = f"index.joint_arith.evals_on_K.{keyfile.EVAL_NAMES[keyfile.EVAL_OF_POLY[v % 6]]}"
+            field = f"index.joint_arith.{label}.polynomial" if v < 6 else ev
+            msg = {1: f"{field}[{i}]: not below the field modulus",
+                   2: f"{ev}[{i}]: not the FFT over K of index.joint_arith.{label}.polynomial",
+                   3: f"index_vk.index_comms[{v}]: not the commitment to index.joint_arith.{label}"}[br.value]
+            raise _lib.B2MError(rc, msg)
+        _lib.check(rc)
+        pk = IndexProverKey(srs, h, types.SimpleNamespace(num_constraints=nc, num_variables=nv, num_instance=ni), self.pc)
+        neg = {}
+        if not marlin:
+            neg = {D - int(b): pts["bound_points"][k].tobytes() for k, b in enumerate(vk["bounds"])}
+        pk.file_g2 = (pts["h"].tobytes(), pts["beta_h"].tobytes(), neg)
+        return pk
+
     # -- prove -----------------------------------------------------------------------------------------
     def prove(self, index_pk, r1cs, zk_rng):
         """[reference src/lib.rs:151-311] -> `CanonicalSerialize` bytes of `Proof<F, PC>`.
@@ -507,25 +844,12 @@ class Marlin:
         """The verifier key of an index: index_info, the six index commitments, g and gamma g, and the verifier's shift
         material for the bounds |H| - 2 and |K| - 2 -- MarlinKZG10: powers_of_g[D - d]; SonicKZG10: beta^-(D - d) h -- with
         h, beta h from the SRS's trapdoor or from the file it was loaded from (as `UniversalSRS.save` takes them)."""
-        from . import srsfile
-        import struct
         L = _lib.lib()
         cid = self.curve_id
         nv, nc, nnz = struct.unpack_from("<QQQ", index_pk.vk_bytes, 0)
-
-        def p2(n):
-            s = 1
-            while s < n:
-                s *= 2
-            return s
-        bounds = sorted({p2(nc) - 2, p2(nnz) - 2})
+        bounds = index_degree_bounds(nc, nnz)
         D = srs.max_degree
-        if srs.trapdoor is not None:
-            h, beta_h, neg = srsfile.g2_setup(cid, fields.FR_MODULUS[cid], srs.trapdoor[0], D, bounds)
-        elif srs.g2 is not None:
-            h, beta_h, neg = srs.g2
-        else:
-            raise ValueError("this SRS has no G2 half (neither a trapdoor nor a source file)")
+        h, beta_h, neg = g2_half(srs, bounds)
         powers = np.ascontiguousarray(srs.powers_limbs)
         if self.pc == _lib.PC_MARLIN_KZG10:
             bound_points = np.ascontiguousarray(np.stack([powers[D - d] for d in bounds]))

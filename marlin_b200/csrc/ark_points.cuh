@@ -1,5 +1,5 @@
-// Batch conversion of ark-serialize G1 / G2 points on the GPU (the SRS loader: b2m_g1_decode_ark, b2m_g2_decode_ark,
-// b2m_g1_to_compressed).  Definitions in ark_points_impl.cuh, instantiated per curve by inst_ark_{bls,bn}.cu.
+// Batch conversion of ark-serialize G1 / G2 points and Fr elements on the GPU (the SRS and index-key loaders:
+// b2m_g1_decode_ark, b2m_g2_decode_ark, b2m_g1_to_compressed, b2m_fr_decode_ark, b2m_fr_to_canonical).  Definitions in ark_points_impl.cuh, instantiated per curve by inst_ark_{bls,bn}.cu.
 #pragma once
 #include "common.cuh"
 #include "field.cuh"
@@ -25,5 +25,16 @@ ArkBad g2_decode_ark(Ctx& cx, const uint8_t* bytes, size_t n, bool compressed, u
 // affine Montgomery limbs -> compressed bytes (sizeof(Fq) each).
 template <class Fq>
 void g1_to_compressed(Ctx& cx, const uint64_t* points_xy, size_t n, uint8_t* out);
+
+// Cause reported by fr_decode_ark for an element that is not below the field modulus.
+constexpr int FR_NOT_CANONICAL = 1;
+
+// n canonical little-endian Fr values (sizeof(Fr) bytes each, host memory) -> Montgomery Fr in DEVICE memory out_dev.
+// Every chunk is decoded; the lowest index of an element >= r over the whole input is returned (index == n: all valid).
+template <class Fr>
+ArkBad fr_decode_ark(Ctx& cx, const uint8_t* bytes, size_t n, Fr* out_dev);
+// n Montgomery Fr in DEVICE memory -> canonical little-endian bytes in host memory.
+template <class Fr>
+void fr_to_canonical(Ctx& cx, const Fr* in_dev, size_t n, uint8_t* out);
 
 }  // namespace b2m

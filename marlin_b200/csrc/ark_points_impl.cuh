@@ -1,4 +1,4 @@
-// Kernels and chunked host drivers of ark_points.cuh.  One thread per point.  Each decode kernel writes the point, its
+// Kernels and chunked host drivers of ark_points.cuh.  One thread per point (or Fr element).  Each decode kernel writes the point, its
 // status, and folds the index of every invalid point into one device word with atomicMin; chunks run in file order and the
 // driver stops at the first chunk with a failure, so the index it reports is the lowest invalid one of the whole input.
 #pragma once
@@ -6,6 +6,7 @@
 
 #include "ark_points.cuh"
 #include "curve.cuh"
+#include "devmem.cuh"
 #include "g1_decode.cuh"
 #include "g2_decode.cuh"
 
@@ -107,9 +108,81 @@ void g1_to_compressed(Ctx& cx, const uint64_t* points_xy, size_t n, uint8_t* out
   }
 }
 
+// ---- Fr elements ------------------------------------------------------------------------------------------------------
+// One thread per element: canonical bytes (staged in device memory) -> check < r -> Montgomery.  `base` is the index of
+// the chunk's first element in the whole input, so one atomicMin word holds the lowest bad index across every chunk.
+template <class Fr>
+__global__ void fr_decode_ark_kernel(const uint8_t* bytes, size_t n, size_t base, Fr* out, unsigned long long* first_bad) {
+  const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  Fr c = ld_fr(reinterpret_cast<const Fr*>(bytes) + i);
+  bool below = false;  // c < r, decided at the highest limb where the two differ (c == r is not below)
+#pragma unroll
+  for (int k = Fr::N - 1; k >= 0; k--) {
+    const uint32_t m = Fr::Params::mod(k);
+    if (c.l[k] != m) {
+      below = c.l[k] < m;
+      break;
+    }
+  }
+  if (!below) {
+    atomicMin(first_bad, (unsigned long long)(base + i));
+    st_fr(out + i, Fr::zero());
+    return;
+  }
+  st_fr(out + i, Fr::from_canonical(c));
+}
+
+template <class Fr>
+__global__ void fr_to_canonical_kernel(const Fr* in, size_t n, Fr* out) {
+  const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  st_fr(out + i, ld_fr(in + i).to_canonical());
+}
+
+template <class Fr>
+ArkBad fr_decode_ark(Ctx& cx, const uint8_t* bytes, size_t n, Fr* out_dev) {
+  if (n == 0) return ArkBad{0, 0};
+  const size_t chunk = std::min(n, ARK_DECODE_CHUNK);
+  DBuf<uint8_t> din(cx, chunk * sizeof(Fr));
+  DBuf<unsigned long long> dbad(cx, 1);
+  B2M_CUDA(cudaMemsetAsync(dbad.p, 0xff, sizeof(unsigned long long), cx.stream));
+  for (size_t at = 0; at < n; at += chunk) {
+    const size_t m = std::min(chunk, n - at);
+    size_t sp = cx.span_begin("ark_h2d", (double)m);
+    din.upload(bytes + at * sizeof(Fr), m * sizeof(Fr));
+    cx.span_end(sp);
+    sp = cx.span_begin("ark_fr_decode", (double)m);
+    fr_decode_ark_kernel<Fr><<<div_up(m, 256), 256, 0, cx.stream>>>(din.p, m, at, out_dev + at, dbad.p);
+    B2M_CHECK_LAUNCH();
+    cx.launches++;
+    cx.span_end(sp);
+  }
+  unsigned long long bad = 0;
+  dbad.download(&bad, 1);
+  return bad == ~0ull ? ArkBad{n, 0} : ArkBad{(size_t)bad, FR_NOT_CANONICAL};
+}
+
+template <class Fr>
+void fr_to_canonical(Ctx& cx, const Fr* in_dev, size_t n, uint8_t* out) {
+  if (n == 0) return;
+  const size_t chunk = std::min(n, ARK_DECODE_CHUNK * 4);
+  DBuf<Fr> dout(cx, chunk);
+  for (size_t at = 0; at < n; at += chunk) {
+    const size_t m = std::min(chunk, n - at);
+    fr_to_canonical_kernel<Fr><<<div_up(m, 256), 256, 0, cx.stream>>>(in_dev + at, m, dout.p);
+    B2M_CHECK_LAUNCH();
+    cx.launches++;
+    dout.download(reinterpret_cast<Fr*>(out) + at, m);
+  }
+}
+
 #define B2M_INSTANTIATE_ARK_POINTS(FQ)                                                                  \
   template ArkBad g1_decode_ark<FQ>(Ctx&, const uint8_t*, size_t, bool, uint64_t*);                  \
   template ArkBad g2_decode_ark<FQ>(Ctx&, const uint8_t*, size_t, bool, uint8_t*);                   \
   template void g1_to_compressed<FQ>(Ctx&, const uint64_t*, size_t, uint8_t*);
+#define B2M_INSTANTIATE_ARK_FR(FR)                                                                      \
+  template ArkBad fr_decode_ark<FR>(Ctx&, const uint8_t*, size_t, FR*);                              \
+  template void fr_to_canonical<FR>(Ctx&, const FR*, size_t, uint8_t*);
 
 }  // namespace b2m

@@ -260,6 +260,106 @@ int b2m_g2_to_compressed(int curve, const uint8_t* uncompressed, size_t n, uint8
 }
 
 }  // extern "C"
+template <class Fr>
+static void fr_decode_host(Ctx& cx, const uint8_t* bytes, size_t n, uint64_t* out, size_t* bad_index) {
+  DBuf<Fr> d(cx, n);
+  const ArkBad bad = fr_decode_ark<Fr>(cx, bytes, n, d.p);
+  if (bad_index) *bad_index = bad.index;
+  if (bad.index != n) throw Error(B2M_ERR_SERIALIZATION, fmt("Fr element %zu: not below the field modulus", bad.index));
+  d.download(reinterpret_cast<Fr*>(out), n);
+  cx.sync();
+}
+template <class Fr>
+static void fr_encode_host(Ctx& cx, const uint64_t* limbs, size_t n, uint8_t* out) {
+  DBuf<Fr> d(cx, n);
+  d.upload(reinterpret_cast<const Fr*>(limbs), n);
+  fr_to_canonical<Fr>(cx, d.p, n, out);
+  cx.sync();
+}
+extern "C" {
+int b2m_fr_decode_ark(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, uint64_t* out_limbs, size_t* bad_index) {
+  return guard([&] {
+    B2M_REQUIRE(ctx && ((bytes && out_limbs) || n == 0), B2M_ERR_INVALID_ARG, "null argument");
+    B2M_REQUIRE(curve == B2M_CURVE_BLS12_381 || curve == B2M_CURVE_BN254, B2M_ERR_INVALID_ARG, "unknown curve id");
+    if (bad_index) *bad_index = n;
+    if (n == 0) return;
+    ctx->cx.use();
+    if (curve == B2M_CURVE_BLS12_381) fr_decode_host<FrBls>(ctx->cx, bytes, n, out_limbs, bad_index);
+    else fr_decode_host<FrBn>(ctx->cx, bytes, n, out_limbs, bad_index);
+  });
+}
+int b2m_fr_to_canonical(b2m_ctx* ctx, int curve, const uint64_t* limbs, size_t n, uint8_t* out) {
+  return guard([&] {
+    B2M_REQUIRE(ctx && ((limbs && out) || n == 0), B2M_ERR_INVALID_ARG, "null argument");
+    B2M_REQUIRE(curve == B2M_CURVE_BLS12_381 || curve == B2M_CURVE_BN254, B2M_ERR_INVALID_ARG, "unknown curve id");
+    if (n == 0) return;
+    ctx->cx.use();
+    if (curve == B2M_CURVE_BLS12_381) fr_encode_host<FrBls>(ctx->cx, limbs, n, out);
+    else fr_encode_host<FrBn>(ctx->cx, limbs, n, out);
+  });
+}
+
+// The row-length chain of an ark-serialize `Vec<Vec<T>>` (host; one step per row, nothing else can be done in parallel)
+int b2m_ark_matrix_rows(const uint8_t* bytes, size_t len, size_t n_rows, size_t entry_bytes, uint64_t* row_ptr, size_t* end,
+                        size_t* bad_row, int* bad_reason) {
+  if (end) *end = 0;
+  if (bad_row) *bad_row = 0;
+  if (bad_reason) *bad_reason = 0;
+  return guard([&] {
+    B2M_REQUIRE(row_ptr && end && (bytes || len == 0) && entry_bytes >= 1, B2M_ERR_INVALID_ARG, "null argument");
+    size_t pos = 0;
+    row_ptr[0] = 0;
+    for (size_t r = 0; r < n_rows; r++) {
+      uint64_t n = 0;
+      if (len - pos < 8) {
+        *end = pos;
+        if (bad_row) *bad_row = r;
+        if (bad_reason) *bad_reason = 1;
+        throw Error(B2M_ERR_SERIALIZATION, fmt("row %zu: truncated in the row length", r));
+      }
+      memcpy(&n, bytes + pos, 8);
+      if (n > (len - pos - 8) / entry_bytes) {
+        *end = pos;
+        if (bad_row) *bad_row = r;
+        if (bad_reason) *bad_reason = 2;
+        throw Error(B2M_ERR_SERIALIZATION, fmt("row %zu: %llu entries run past the end", r, (unsigned long long)n));
+      }
+      row_ptr[r + 1] = row_ptr[r] + n;
+      pos += 8 + n * entry_bytes;
+    }
+    *end = pos;
+  });
+}
+
+}  // extern "C"
+// `Radix2EvaluationDomain::new(2^log_size)` as ark-serialize writes it [U ark-poly 0.3 domain/radix2]
+template <class Fr>
+static void domain_ark_impl(unsigned log_size, uint8_t* out) {
+  B2M_REQUIRE((int)log_size <= Fr::Params::TWO_ADICITY, B2M_ERR_DEGREE_TOO_LARGE, "2^%u exceeds the 2-adicity of the field", log_size);
+  const uint64_t size = (uint64_t)1 << log_size;
+  const uint32_t lg = log_size;
+  memcpy(out, &size, 8);
+  memcpy(out + 8, &lg, 4);
+  Fr gen;
+  for (int i = 0; i < Fr::N; i++) gen.l[i] = Fr::Params::gen(i);
+  const Fr size_f = Fr::from_u64(size), w = Ntt<Fr>::root_of_unity((int)log_size);
+  const Fr vals[5] = {size_f, size_f.inverse(), w, w.inverse(), gen.inverse()};
+  for (int k = 0; k < 5; k++) {
+    const Fr c = vals[k].to_canonical();
+    memcpy(out + 12 + k * sizeof(Fr), c.l, sizeof(Fr));
+  }
+}
+extern "C" {
+int b2m_domain_ark(int curve, unsigned log_size, uint8_t* out) {
+  return guard([&] {
+    B2M_REQUIRE(out != nullptr, B2M_ERR_INVALID_ARG, "null argument");
+    if (curve == B2M_CURVE_BLS12_381) domain_ark_impl<FrBls>(log_size, out);
+    else if (curve == B2M_CURVE_BN254) domain_ark_impl<FrBn>(log_size, out);
+    else throw Error(B2M_ERR_INVALID_ARG, "unknown curve id");
+  });
+}
+
+}  // extern "C"
 // standard G2 generators (canonical x.c0, x.c1, y.c0, y.c1; big-endian hex), checked on-curve / order r in tests/test_srs_files.py
 static const char* const G2_GEN_BLS[4] = {
     "024aa2b2f08f0a91260805272dc51051c6e47ad4fa403b02b4510b647ae3d1770bac0326a805bbefd48056c8c121bdb8",
@@ -487,6 +587,48 @@ int b2m_index_create(b2m_srs* srs, int pc_variant, size_t num_constraints, size_
       idx->impl.reset(make_index_bn(srs, pc_variant, num_constraints, num_variables, num_instance_variables, a, b, c));
     *out = idx.release();
     srs->children++;
+  });
+}
+
+int b2m_index_load(b2m_srs* srs, int pc_variant, size_t num_constraints, size_t num_variables, size_t num_instance_variables,
+                   size_t num_non_zero, const b2m_matrix* a, const b2m_matrix* b, const b2m_matrix* c, const uint8_t* const* vectors,
+                   const size_t* vector_lens, const uint64_t* index_comms_xy, int check_commitments, size_t* bad_vector, size_t* bad_index,
+                   int* bad_reason, b2m_index** out) {
+  size_t bad[3] = {0, 0, 0};
+  const int rc = guard([&] {
+    B2M_REQUIRE(srs && a && b && c && vectors && vector_lens && index_comms_xy && out, B2M_ERR_INVALID_ARG, "null argument");
+    B2M_REQUIRE(pc_variant == B2M_PC_MARLIN_KZG10 || pc_variant == B2M_PC_SONIC_KZG10, B2M_ERR_INVALID_ARG, "unknown PC variant");
+    for (int v = 0; v < 12; v++) B2M_REQUIRE(vectors[v] || vector_lens[v] == 0, B2M_ERR_INVALID_ARG, "index vector %d is null", v);
+    srs->ctx->cx.use();
+    std::unique_ptr<b2m_index> idx(new b2m_index);
+    idx->srs = srs;
+    if (srs->curve == B2M_CURVE_BLS12_381)
+      idx->impl.reset(load_index_bls(srs, pc_variant, num_constraints, num_variables, num_instance_variables, num_non_zero, a, b, c, vectors,
+                                     vector_lens, index_comms_xy, check_commitments != 0, bad));
+    else
+      idx->impl.reset(load_index_bn(srs, pc_variant, num_constraints, num_variables, num_instance_variables, num_non_zero, a, b, c, vectors,
+                                    vector_lens, index_comms_xy, check_commitments != 0, bad));
+    *out = idx.release();
+    srs->children++;
+  });
+  if (bad_vector) *bad_vector = bad[0];
+  if (bad_index) *bad_index = bad[1];
+  if (bad_reason) *bad_reason = rc == B2M_ERR_SERIALIZATION ? (int)bad[2] : 0;
+  return rc;
+}
+
+int b2m_index_sizes(const b2m_index* idx, size_t* num_non_zero, size_t* domain_k, size_t* matrix_nnz) {
+  return guard([&] {
+    B2M_REQUIRE(idx && num_non_zero && domain_k && matrix_nnz, B2M_ERR_INVALID_ARG, "null argument");
+    idx->impl->sizes(num_non_zero, domain_k, matrix_nnz);
+  });
+}
+
+int b2m_index_export(b2m_index* idx, uint8_t* vectors, uint64_t* const* row_ptrs, uint64_t* const* cols, uint8_t* const* coeffs) {
+  return guard([&] {
+    B2M_REQUIRE(idx != nullptr, B2M_ERR_INVALID_ARG, "null argument");
+    idx->srs->ctx->cx.use();
+    idx->impl->export_keys(vectors, row_ptrs, cols, coeffs);
   });
 }
 

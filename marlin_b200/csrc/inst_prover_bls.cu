@@ -6,6 +6,20 @@ IndexBase* make_index_bls(b2m_srs* srs, int pc, size_t nc, size_t nv, size_t ni,
   idx->build(a, b, c);
   return idx.release();
 }
+IndexBase* load_index_bls(b2m_srs* srs, int pc, size_t nc, size_t nv, size_t ni, size_t nnz, const b2m_matrix* a, const b2m_matrix* b,
+                          const b2m_matrix* c, const uint8_t* const* vectors, const size_t* lens, const uint64_t* comms_xy, bool check_commitments,
+                          size_t bad[3]) {
+  using I = MarlinIndex<FrBls, FqBls>;
+  std::unique_ptr<I> idx(new I(srs, srs->ctx->ntt_bls(), *srs->bls, pc, nc, nv, ni));
+  typename I::LoadBad lb{0, 0, 0};
+  try {
+    idx->load(a, b, c, nnz, vectors, lens, comms_xy, check_commitments, &lb);
+  } catch (...) {
+    bad[0] = lb.vector; bad[1] = lb.index; bad[2] = (size_t)lb.reason;
+    throw;
+  }
+  return idx.release();
+}
 void pc_commit_bls(b2m_srs* srs, int pc, size_t n_polys, const uint64_t* const* coeffs, const size_t* n_coeffs,
                    const int64_t* degree_bounds, const int64_t* hiding_bounds, b2m_rng* rng, uint64_t* out_comm_xy, uint64_t* out_shifted_xy,
                    uint64_t* out_rand, uint64_t* out_shifted_rand, size_t rand_stride) {

@@ -16,6 +16,10 @@ struct IndexBase {
                      std::vector<uint8_t>& proof) = 0;
   // Copy an instance (x, w) into HBM ahead of time; a later prove() with null pointers uses it.
   virtual void stage(const uint64_t* formatted_input, size_t n_input, const uint64_t* witness, size_t n_witness) = 0;
+  // joint non-zeros, |K| and the entries of A, B, C (b2m_index_sizes)
+  virtual void sizes(size_t* num_non_zero, size_t* domain_k, size_t* matrix_nnz) const = 0;
+  // b2m_index_export
+  virtual void export_keys(uint8_t* vectors, uint64_t* const* row_ptrs, uint64_t* const* cols, uint8_t* const* coeffs) = 0;
   std::vector<uint8_t> vk_bytes;    // IndexVerifierKey::write (ToBytes)
   std::vector<uint64_t> comms_xy;   // six index commitments, affine Montgomery limbs
   std::string timings_json;
@@ -25,6 +29,14 @@ IndexBase* make_index_bls(b2m_srs* srs, int pc, size_t num_constraints, size_t n
                           const b2m_matrix* a, const b2m_matrix* b, const b2m_matrix* c);
 IndexBase* make_index_bn(b2m_srs* srs, int pc, size_t num_constraints, size_t num_variables, size_t num_instance,
                          const b2m_matrix* a, const b2m_matrix* b, const b2m_matrix* c);
+
+// An index from a key file (b2m_index_load).  bad receives (vector, index, reason) of the first failed check.
+IndexBase* load_index_bls(b2m_srs* srs, int pc, size_t num_constraints, size_t num_variables, size_t num_instance, size_t num_non_zero,
+                          const b2m_matrix* a, const b2m_matrix* b, const b2m_matrix* c, const uint8_t* const* vectors, const size_t* lens,
+                          const uint64_t* comms_xy, bool check_commitments, size_t bad[3]);
+IndexBase* load_index_bn(b2m_srs* srs, int pc, size_t num_constraints, size_t num_variables, size_t num_instance, size_t num_non_zero,
+                         const b2m_matrix* a, const b2m_matrix* b, const b2m_matrix* c, const uint8_t* const* vectors, const size_t* lens,
+                         const uint64_t* comms_xy, bool check_commitments, size_t bad[3]);
 
 // `PC::commit` over host polynomials (Level 1 of include/b2m.h)
 void pc_commit_bls(b2m_srs* srs, int pc, size_t n_polys, const uint64_t* const* coeffs, const size_t* n_coeffs,

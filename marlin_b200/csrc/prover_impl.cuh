@@ -16,6 +16,7 @@
 #include <chrono>
 #include <cstring>
 
+#include "ark_points.cuh"
 #include "capi_types.cuh"
 #include "hostutil.hpp"
 #include "pc_impl.cuh"
@@ -102,52 +103,31 @@ struct MarlinIndex : IndexBase {
   MarlinIndex(b2m_srs* s, Ntt<Fr>& ntt_, Msm<Fr, Fq>& msm_, int pc_, size_t nc_, size_t nv_, size_t ni_)
       : srs(s), cx(s->ctx->cx), ntt(ntt_), msm(msm_), pc(pc_), nc(nc_), nv(nv_), ni(ni_) {}
 
-  // (extended device lambdas may not live in a constructor, hence a separate build step)
-  void build(const b2m_matrix* a, const b2m_matrix* b, const b2m_matrix* c) {
+  // The matrices as the index received them (row form, Montgomery coefficients): kept for export (b2m_index_export).
+  std::vector<uint64_t> m_rowptr[3], m_col[3], m_coeff[3];
+
+  // Checks the dimensions and builds every structure derived from the matrices alone, in both the `Marlin::index` path
+  // (build) and the key-file path (load): the host copies above, the CSR of A and B for z_A, z_B, and the column buckets
+  // of A, B, C for t(X).
+  void prepare(const b2m_matrix* a, const b2m_matrix* b, const b2m_matrix* c) {
     B2M_REQUIRE(nc == nv, B2M_ERR_NON_SQUARE, "matrices are not square: %zu constraints, %zu variables", nc, nv);
     B2M_REQUIRE(is_pow2(ni), B2M_ERR_INVALID_PUBLIC_INPUT_LEN, "formatted public input length %zu is not a power of two", ni);
     B2M_REQUIRE(nc >= 1 && ni <= nv, B2M_ERR_INVALID_ARG, "bad dimensions");
-    const int S = Fr::Params::TWO_ADICITY;
     log_h = log2_ceil(nc); log_x = log2_ceil(ni);
     H = (size_t)1 << log_h; X = ni;  // X <= nv = nc <= H
     // |X| == |H| (only public inputs, no witness) is a valid index, as in the reference: every column is then an input
     // column, so reindex() maps i -> i, w(X) is the constant rho_w and z(X) = rho_w v_X(X) + x(X).
-
-    // joint matrix (sorted union of the column sets per row) [reference indexer.rs:83-102]
-    std::vector<uint32_t> jr, jc;
-    std::vector<Fr> va, vb, vc;
-    std::vector<uint64_t> cols;
     const b2m_matrix* ms[3] = {a, b, c};
-    for (size_t r = 0; r < nc; r++) {
-      cols.clear();
-      for (int m = 0; m < 3; m++)
-        for (uint64_t e = ms[m]->row_ptr[r]; e < ms[m]->row_ptr[r + 1]; e++) {
-          B2M_REQUIRE(ms[m]->col[e] < nv, B2M_ERR_INVALID_ARG, "column index %llu out of range", (unsigned long long)ms[m]->col[e]);
-          cols.push_back(ms[m]->col[e]);
-        }
-      std::sort(cols.begin(), cols.end());
-      cols.erase(std::unique(cols.begin(), cols.end()), cols.end());
-      for (uint64_t col : cols) {
-        jr.push_back((uint32_t)r);
-        jc.push_back((uint32_t)reindex(col));
-        Fr v[3];
-        for (int m = 0; m < 3; m++) {
-          v[m] = Fr::zero();
-          for (uint64_t e = ms[m]->row_ptr[r]; e < ms[m]->row_ptr[r + 1]; e++)
-            if (ms[m]->col[e] == col) v[m] = fr_from_limbs(ms[m]->coeff + 4 * e);  // BTreeMap collect: last wins
-        }
-        va.push_back(v[0]); vb.push_back(v[1]); vc.push_back(v[2]);
-      }
+    for (int m = 0; m < 3; m++) {
+      const size_t ne = ms[m]->row_ptr[nc];
+      for (size_t r = 0; r < nc; r++)
+        B2M_REQUIRE(ms[m]->row_ptr[r] <= ms[m]->row_ptr[r + 1], B2M_ERR_INVALID_ARG, "matrix %d: row pointers decrease at row %zu", m, r);
+      for (size_t e = 0; e < ne; e++)
+        B2M_REQUIRE(ms[m]->col[e] < nv, B2M_ERR_INVALID_ARG, "column index %llu out of range", (unsigned long long)ms[m]->col[e]);
+      m_rowptr[m].assign(ms[m]->row_ptr, ms[m]->row_ptr + nc + 1);
+      m_col[m].assign(ms[m]->col, ms[m]->col + ne);
+      m_coeff[m].assign(ms[m]->coeff, ms[m]->coeff + 4 * ne);
     }
-    nnz = jr.size();
-    B2M_REQUIRE(nnz >= 1, B2M_ERR_INVALID_ARG, "empty constraint matrices");
-    log_k = log2_ceil(nnz);
-    K = (size_t)1 << log_k;
-    B2M_REQUIRE(log_k + 1 <= S && log_h + 2 <= S, B2M_ERR_DEGREE_TOO_LARGE, "domains exceed the field's 2-adicity");
-    D = srs->n_g - 1;
-    size_t md = std::max(std::max(2 * H - 1, 3 * H - 1), K - 1);  // reference src/ahp/mod.rs:83-92 with zk_bound = 1
-    B2M_REQUIRE(D >= md, B2M_ERR_INDEX_TOO_LARGE, "SRS max degree %zu < index max degree %zu", D, md);
-    B2M_REQUIRE(D >= K - 2 && D >= H - 2, B2M_ERR_INDEX_TOO_LARGE, "SRS too small for the degree bounds");
 
     // CSR copies of A and B for z_A = A z, z_B = B z  [reference prover.rs:256-276]
     auto upload_csr = [&](const b2m_matrix* m, DBuf<uint32_t>& rp, DBuf<uint32_t>& cl, DBuf<Fr>& cf) {
@@ -185,9 +165,69 @@ struct MarlinIndex : IndexBase {
       t_mat.upload(hmat.data(), hmat.size()); t_coeff.upload(hco.data(), hco.size());
       cx.sync();
     }
+  }
+
+  // |K| from the joint non-zero count, and the SRS checks of `Marlin::index`
+  void set_k(size_t nnz_) {
+    nnz = nnz_;
+    B2M_REQUIRE(nnz >= 1, B2M_ERR_INVALID_ARG, "empty constraint matrices");
+    log_k = log2_ceil(nnz);
+    K = (size_t)1 << log_k;
+    const int S = Fr::Params::TWO_ADICITY;
+    B2M_REQUIRE(log_k + 1 <= S && log_h + 2 <= S, B2M_ERR_DEGREE_TOO_LARGE, "domains exceed the field's 2-adicity");
+    D = srs->n_g - 1;
+    size_t md = std::max(std::max(2 * H - 1, 3 * H - 1), K - 1);  // reference src/ahp/mod.rs:83-92 with zk_bound = 1
+    B2M_REQUIRE(D >= md, B2M_ERR_INDEX_TOO_LARGE, "SRS max degree %zu < index max degree %zu", D, md);
+    B2M_REQUIRE(D >= K - 2 && D >= H - 2, B2M_ERR_INDEX_TOO_LARGE, "SRS too small for the degree bounds");
+    ntt.ensure_table(std::max(log_k + 1, log_h + 2));
+    for (int i = 0; i < 6; i++) { ieval[i] = DBuf<Fr>(cx, K); ipoly[i] = DBuf<Fr>(cx, K); }
+  }
+
+  // the six index polynomials as PC inputs, their commitments, and `IndexVerifierKey::write` (ToBytes): index_info (3 x u64)
+  // || index_comms  [reference data_structures.rs:36-43, indexer.rs:63-69]
+  void finish_vk() {
+    comms_xy.resize(6 * 2 * LQ);
+    for (int i = 0; i < 6; i++) memcpy(comms_xy.data() + i * 2 * LQ, &index_polys[i].comm, sizeof(Pt));
+    vk_bytes.clear();
+    put_u64(vk_bytes, nv); put_u64(vk_bytes, nc); put_u64(vk_bytes, nnz);
+    for (int i = 0; i < 6; i++) write_commitment(vk_bytes, index_polys[i].comm, false, Pt::inf());
+  }
+  void bind_index_polys() {
+    for (int i = 0; i < 6; i++) {
+      index_polys[i].p = ipoly[i].p;
+      index_polys[i].len = K;
+    }
+  }
+
+  // (extended device lambdas may not live in a constructor, hence a separate build step)
+  void build(const b2m_matrix* a, const b2m_matrix* b, const b2m_matrix* c) {
+    prepare(a, b, c);
+    // joint matrix (sorted union of the column sets per row) [reference indexer.rs:83-102]
+    std::vector<uint32_t> jr, jc;
+    std::vector<Fr> va, vb, vc;
+    std::vector<uint64_t> cols;
+    const b2m_matrix* ms[3] = {a, b, c};
+    for (size_t r = 0; r < nc; r++) {
+      cols.clear();
+      for (int m = 0; m < 3; m++)
+        for (uint64_t e = ms[m]->row_ptr[r]; e < ms[m]->row_ptr[r + 1]; e++) cols.push_back(ms[m]->col[e]);
+      std::sort(cols.begin(), cols.end());
+      cols.erase(std::unique(cols.begin(), cols.end()), cols.end());
+      for (uint64_t col : cols) {
+        jr.push_back((uint32_t)r);
+        jc.push_back((uint32_t)reindex(col));
+        Fr v[3];
+        for (int m = 0; m < 3; m++) {
+          v[m] = Fr::zero();
+          for (uint64_t e = ms[m]->row_ptr[r]; e < ms[m]->row_ptr[r + 1]; e++)
+            if (ms[m]->col[e] == col) v[m] = fr_from_limbs(ms[m]->coeff + 4 * e);  // BTreeMap collect: last wins
+        }
+        va.push_back(v[0]); vb.push_back(v[1]); vc.push_back(v[2]);
+      }
+    }
+    set_k(jr.size());
 
     // arithmetization of M* on the device [reference constraint_systems.rs:125-262]
-    ntt.ensure_table(std::max(log_k + 1, log_h + 2));
     const Fr* tw = ntt.table.tw;
     const int ml = ntt.table.max_log, lh = log_h;
     {
@@ -195,7 +235,6 @@ struct MarlinIndex : IndexBase {
       DBuf<Fr> dva(cx, nnz), dvb(cx, nnz), dvc(cx, nnz);
       djr.upload(jr.data(), nnz); djc.upload(jc.data(), nnz);
       dva.upload(va.data(), nnz); dvb.upload(vb.data(), nnz); dvc.upload(vc.data(), nnz);
-      for (int i = 0; i < 6; i++) { ieval[i] = DBuf<Fr>(cx, K); ipoly[i] = DBuf<Fr>(cx, K); }
       Fr* e_row = ieval[0].p; Fr* e_col = ieval[1].p; Fr* e_a = ieval[2].p; Fr* e_b = ieval[3].p; Fr* e_c = ieval[4].p;
       Fr* e_rc = ieval[5].p;
       const uint32_t* pjr = djr.p; const uint32_t* pjc = djc.p;
@@ -226,19 +265,110 @@ struct MarlinIndex : IndexBase {
       cx.sync();
     }
     // commit to the index polynomials, rng = None [reference lib.rs:124-125]
+    bind_index_polys();
     std::vector<LP*> ips;
-    for (int i = 0; i < 6; i++) {
-      index_polys[i].p = ipoly[i].p;
-      index_polys[i].len = K;
-      ips.push_back(&index_polys[i]);
-    }
+    for (int i = 0; i < 6; i++) ips.push_back(&index_polys[i]);
     ZkSource<b2m_rng> no_rng(nullptr);
     pc_commit(srs, msm, pc, ips, no_rng);
-    comms_xy.resize(6 * 2 * LQ);
-    for (int i = 0; i < 6; i++) memcpy(comms_xy.data() + i * 2 * LQ, &index_polys[i].comm, sizeof(Pt));
-    // IndexVerifierKey::write: index_info (3 x u64) || index_comms  [reference data_structures.rs:36-43, indexer.rs:63-69]
-    put_u64(vk_bytes, nv); put_u64(vk_bytes, nc); put_u64(vk_bytes, nnz);
-    for (int i = 0; i < 6; i++) write_commitment(vk_bytes, index_polys[i].comm, false, Pt::inf());
+    finish_vk();
+  }
+
+  // An index from a key file (b2m_index_load): the matrices give the same derived structures as build(); the twelve index
+  // vectors (coefficients, then evaluations on K, each in the order row, col, a_val, b_val, c_val, row_col) are decoded on
+  // the device straight into the index's buffers, with no arithmetization and no commitment MSM.  What is checked on the
+  // device: every element is below r, and the NTT over K of each zero-padded coefficient vector equals its evaluations;
+  // with check_commitments the six commitments are recomputed and compared.  The first failure is reported in *bad
+  // (vector 0..11, index, reason: 1 not below r, 2 coefficients and evaluations differ, 3 commitment differs).
+  struct LoadBad {
+    size_t vector, index;
+    int reason;
+  };
+  void load(const b2m_matrix* a, const b2m_matrix* b, const b2m_matrix* c, size_t nnz_, const uint8_t* const* vectors,
+            const size_t* lens, const uint64_t* comms, bool check_commitments, LoadBad* bad) {
+    prepare(a, b, c);
+    // the joint matrix is the union of the three: at least as many entries as each, at most as many as all of them
+    size_t most = 0, total = 0;
+    for (int m = 0; m < 3; m++) {
+      most = std::max(most, m_col[m].size());
+      total += m_col[m].size();
+    }
+    B2M_REQUIRE(nnz_ >= most && nnz_ <= total, B2M_ERR_INVALID_ARG, "num_non_zero %zu is outside [%zu, %zu], the range the matrices allow", nnz_,
+                most, total);
+    set_k(nnz_);
+    for (int i = 0; i < 6; i++) {
+      B2M_REQUIRE(lens[i] <= K, B2M_ERR_INVALID_ARG, "index polynomial %d has %zu coefficients, |K| = %zu", i, lens[i], K);
+      B2M_REQUIRE(lens[6 + i] == K, B2M_ERR_INVALID_ARG, "index evaluation vector %d has %zu elements, |K| = %zu", i, lens[6 + i], K);
+    }
+    auto fail = [&](size_t v, size_t at, int reason, const char* what) {
+      *bad = LoadBad{v, at, reason};
+      throw Error(B2M_ERR_SERIALIZATION, fmt("index vector %zu, element %zu: %s", v, at, what));
+    };
+    for (int v = 0; v < 12; v++) {
+      Fr* dst = v < 6 ? ipoly[v].p : ieval[v - 6].p;
+      const ArkBad r = fr_decode_ark<Fr>(cx, vectors[v], lens[v], dst);
+      if (r.index != lens[v]) fail(v, r.index, 1, "not below the field modulus");
+      if (v < 6 && lens[v] < K) B2M_CUDA(cudaMemsetAsync(dst + lens[v], 0, (K - lens[v]) * sizeof(Fr), cx.stream));
+    }
+    // evals_on_K == FFT_K(coefficients): one compare kernel per polynomial, the lowest mismatch of each in its own word
+    {
+      DBuf<unsigned long long> first(cx, 6);
+      B2M_CUDA(cudaMemsetAsync(first.p, 0xff, 6 * sizeof(unsigned long long), cx.stream));
+      DBuf<Fr> ev(cx, K);
+      for (int i = 0; i < 6; i++) {
+        fft_padded(ipoly[i].p, K, log_k, ev.p);
+        const Fr* got = ev.p; const Fr* want = ieval[i].p;
+        unsigned long long* slot = first.p + i;
+        ew(cx, K, [=] __device__(size_t k) {
+          if (ld_fr(got + k) != ld_fr(want + k)) atomicMin(slot, (unsigned long long)k);
+        });
+      }
+      unsigned long long h[6];
+      first.download(h, 6);
+      for (int i = 0; i < 6; i++)
+        if (h[i] != ~0ull) fail(6 + i, (size_t)h[i], 2, "the evaluations are not the FFT of the coefficients");
+    }
+    bind_index_polys();
+    for (int i = 0; i < 6; i++) memcpy(&index_polys[i].comm, comms + i * 2 * LQ, sizeof(Pt));
+    if (check_commitments) {
+      LP fresh[6];
+      std::vector<LP*> ips;
+      for (int i = 0; i < 6; i++) {
+        fresh[i].p = ipoly[i].p;
+        fresh[i].len = K;
+        ips.push_back(&fresh[i]);
+      }
+      ZkSource<b2m_rng> no_rng(nullptr);
+      pc_commit(srs, msm, pc, ips, no_rng);
+      for (int i = 0; i < 6; i++)
+        if (memcmp(&fresh[i].comm, &index_polys[i].comm, sizeof(Pt)) != 0) {
+          *bad = LoadBad{(size_t)i, 0, 3};
+          throw Error(B2M_ERR_SERIALIZATION, fmt("index commitment %d differs from the commitment to its polynomial", i));
+        }
+    }
+    finish_vk();
+  }
+
+  void sizes(size_t* out_nnz, size_t* out_k, size_t* matrix_nnz) const override {
+    *out_nnz = nnz;
+    *out_k = K;
+    for (int m = 0; m < 3; m++) matrix_nnz[m] = m_col[m].size();
+  }
+  // b2m_index_export: the twelve vectors (K canonical Fr each, coefficients zero-padded) and the matrices in row form with
+  // canonical coefficients, both converted on the device
+  void export_keys(uint8_t* vectors, uint64_t* const* row_ptrs, uint64_t* const* cols, uint8_t* const* coeffs) override {
+    if (vectors)
+      for (int v = 0; v < 12; v++) fr_to_canonical<Fr>(cx, v < 6 ? ipoly[v].p : ieval[v - 6].p, K, vectors + (size_t)v * K * sizeof(Fr));
+    for (int m = 0; m < 3; m++) {
+      if (row_ptrs && row_ptrs[m]) memcpy(row_ptrs[m], m_rowptr[m].data(), m_rowptr[m].size() * sizeof(uint64_t));
+      if (cols && cols[m]) memcpy(cols[m], m_col[m].data(), m_col[m].size() * sizeof(uint64_t));
+      const size_t ne = m_col[m].size();
+      if (coeffs && coeffs[m] && ne) {
+        DBuf<Fr> d(cx, ne);
+        d.upload(reinterpret_cast<const Fr*>(m_coeff[m].data()), ne);
+        fr_to_canonical<Fr>(cx, d.p, ne, coeffs[m]);
+      }
+    }
+    cx.sync();
   }
 
   // ---- ToBytes / CanonicalSerialize of group and field elements (SURVEY.md A.2 / A.3) ------------

@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """Writes the replay kit tools/replay_rs consumes (needs a GPU): an SRS file in ark-serialize layout, and -- for MarlinKZG10 and
-SonicKZG10 -- the `ToBytes` image of index_vk and the `CanonicalSerialize` bytes of a proof of the reference bench's DummyCircuit,
-all produced by libb2m.so, plus the inputs in meta.json.   python tools/make_replay_kit.py tests/golden/replay_kit [log_n]"""
+SonicKZG10 -- the `ToBytes` image of index_vk, the `CanonicalSerialize` bytes of a proof of the reference bench's DummyCircuit and
+the index key files (`IndexProverKey` / `IndexVerifierKey` `serialize`, marlin_b200/keyfile.py), all produced by libb2m.so, plus the inputs in meta.json.   python tools/make_replay_kit.py tests/golden/replay_kit [log_n]"""
 import json
 import os
 import sys
@@ -36,6 +36,8 @@ def main():
         proof = m.prove(pk, circ, rng)
         open(os.path.join(out, f"{pc}_index_vk_tobytes.bin"), "wb").write(pk.vk_bytes)
         open(os.path.join(out, f"{pc}_proof.bin"), "wb").write(proof)
+        pk.save(os.path.join(out, f"{pc}_index_pk.bin"), compressed=True)  # IndexProverKey / IndexVerifierKey `serialize`
+        pk.save_verifier_key(os.path.join(out, f"{pc}_index_vk.bin"), compressed=True)
         meta["zk_word_pos_after"][pc] = rng.word_pos
         pk.close()
     srs.close()

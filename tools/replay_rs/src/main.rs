@@ -81,7 +81,49 @@ where PC: PolynomialCommitment<Fr, DensePolynomial<Fr>> {
     let gpu_proof = ark_marlin::Proof::<Fr, PC>::deserialize(&want_proof[..]).expect("deserialize the kit's proof");
     let ok_gpu = Marlin::<Fr, PC, FS>::verify(&vk, &[c], &gpu_proof, &mut ChaCha12Rng::from_seed([7u8; 32])).unwrap_or(false);
     println!("{}: the kit's proof is accepted by ark-marlin: {}", scheme, ok_gpu);
-    got_vk == want_vk && got_proof == want_proof && zk.get_word_pos() == want_pos && ok_verify && ok_gpu
+    let ok_keys = replay_key_files::<PC>(dir, scheme, &pk, &vk, circ, &c);
+    got_vk == want_vk && got_proof == want_proof && zk.get_word_pos() == want_pos && ok_verify && ok_gpu && ok_keys
+}
+
+// Index key files (IndexProverKey::save / save_verifier_key, compressed form; marlin_b200/keyfile.py): each file must
+// `deserialize` into the real arkworks type, serialize back to the same bytes, and equal this run's own `Marlin::index`
+// output byte for byte -- the check that pins the recalled layouts.  A kit without the files skips the check.
+fn replay_key_files<PC>(dir: &str, scheme: &str, pk: &ark_marlin::IndexProverKey<Fr, PC>, vk: &ark_marlin::IndexVerifierKey<Fr, PC>,
+                        circ: DummyCircuit, c: &Fr) -> bool
+where PC: PolynomialCommitment<Fr, DensePolynomial<Fr>> {
+    let pk_path = format!("{}/{}_index_pk.bin", dir, scheme);
+    let vk_path = format!("{}/{}_index_vk.bin", dir, scheme);
+    let (file_pk, file_vk) = match (std::fs::read(&pk_path), std::fs::read(&vk_path)) {
+        (Ok(p), Ok(v)) => (p, v),
+        _ => {
+            println!("{}: no index key files in the kit, skipped", scheme);
+            return true;
+        }
+    };
+    let mut own_pk = Vec::new();
+    pk.serialize(&mut own_pk).unwrap();
+    let mut own_vk = Vec::new();
+    vk.serialize(&mut own_vk).unwrap();
+    let read_pk = ark_marlin::IndexProverKey::<Fr, PC>::deserialize(&file_pk[..]);
+    let read_vk = ark_marlin::IndexVerifierKey::<Fr, PC>::deserialize(&file_vk[..]);
+    let round_pk = read_pk.as_ref().map(|k| { let mut b = Vec::new(); k.serialize(&mut b).unwrap(); b == file_pk }).unwrap_or(false);
+    let round_vk = read_vk.as_ref().map(|k| { let mut b = Vec::new(); k.serialize(&mut b).unwrap(); b == file_vk }).unwrap_or(false);
+    let first_diff = |a: &[u8], b: &[u8]| a.iter().zip(b).position(|(x, y)| x != y).unwrap_or(a.len().min(b.len()));
+    println!("{}: index_pk file deserializes {} | round trip {} | equals Marlin::index {} (first difference at byte {} of {} / {})",
+             scheme, read_pk.is_ok(), round_pk, own_pk == file_pk, first_diff(&own_pk, &file_pk), own_pk.len(), file_pk.len());
+    println!("{}: index_vk file deserializes {} | round trip {} | equals Marlin::index {} (first difference at byte {} of {} / {})",
+             scheme, read_vk.is_ok(), round_vk, own_vk == file_vk, first_diff(&own_vk, &file_vk), own_vk.len(), file_vk.len());
+    // the deserialized verifier key verifies a proof made with the deserialized prover key
+    let ok_use = match (read_pk, read_vk) {
+        (Ok(rpk), Ok(rvk)) => {
+            let mut zk = ChaCha12Rng::from_seed([9u8; 32]);
+            let proof = Marlin::<Fr, PC, FS>::prove(&rpk, circ, &mut zk).expect("prove with the file's key");
+            Marlin::<Fr, PC, FS>::verify(&rvk, &[*c], &proof, &mut ChaCha12Rng::from_seed([7u8; 32])).unwrap_or(false)
+        }
+        _ => false,
+    };
+    println!("{}: a proof made with the file's prover key verifies under the file's verifier key: {}", scheme, ok_use);
+    round_pk && round_vk && own_pk == file_pk && own_vk == file_vk && ok_use
 }
 
 fn main() {
