@@ -52,6 +52,8 @@ pub const B2M_ERR_MISSING_RNG: c_int = 7;
 pub const B2M_ERR_CUDA: c_int = 8;
 pub const B2M_ERR_NCCL: c_int = 9;
 pub const B2M_ERR_UNSUPPORTED: c_int = 10;
+pub const B2M_ERR_SERIALIZATION: c_int = 11;
+pub const B2M_ERR_MEMORY_LIMIT: c_int = 12;
 pub const B2M_CURVE_BLS12_381: c_int = 0;
 pub const B2M_CURVE_BN254: c_int = 1;
 pub const B2M_PC_MARLIN_KZG10: c_int = 0;
@@ -63,6 +65,8 @@ extern "C" {
     pub fn b2m_ctx_create(device: c_int, out: *mut *mut b2m_ctx) -> c_int;
     pub fn b2m_ctx_destroy(ctx: *mut b2m_ctx);
     pub fn b2m_ctx_launches(ctx: *const b2m_ctx) -> c_ulonglong;
+    pub fn b2m_ctx_set_memory_limit(ctx: *mut b2m_ctx, bytes: usize) -> c_int;
+    pub fn b2m_ctx_memory(ctx: *mut b2m_ctx, out: *mut usize) -> c_int;
     pub fn b2m_comm_unique_id(id: *mut u8, cap: usize) -> c_int;
     pub fn b2m_ctx_attach_comm(ctx: *mut b2m_ctx, id: *const u8, id_len: usize, rank: c_int, world: c_int) -> c_int;
     pub fn b2m_ntt(ctx: *mut b2m_ctx, curve: c_int, data: *mut u64, log_n: c_uint, inverse: c_int, coset: c_int) -> c_int;
@@ -70,8 +74,13 @@ extern "C" {
                       out_is_inf: *mut c_int) -> c_int;
     pub fn b2m_srs_create(ctx: *mut b2m_ctx, curve: c_int, powers_of_g: *const u64, n_g: usize, powers_of_gamma_g: *const u64,
                           gamma_indices: *const u64, n_gamma: usize, window_bits: c_int, out: *mut *mut b2m_srs) -> c_int;
+    pub fn b2m_srs_create_layout(ctx: *mut b2m_ctx, curve: c_int, powers_of_g: *const u64, n_g: usize, powers_of_gamma_g: *const u64,
+                                 gamma_indices: *const u64, n_gamma: usize, window_bits: c_int, window_tables: c_int,
+                                 out: *mut *mut b2m_srs) -> c_int;
     pub fn b2m_srs_destroy(srs: *mut b2m_srs);
     pub fn b2m_srs_size(srs: *const b2m_srs) -> usize;
+    pub fn b2m_srs_window_tables(srs: *const b2m_srs) -> c_int;
+    pub fn b2m_srs_layout(srs: *const b2m_srs, out: *mut usize) -> c_int;
     pub fn b2m_srs_msm(srs: *mut b2m_srs, base_off: usize, scalars: *const u64, n: usize, out_xy: *mut u64, out_is_inf: *mut c_int) -> c_int;
     pub fn b2m_pc_commit(srs: *mut b2m_srs, pc_variant: c_int, n_polys: usize, coeffs: *const *const u64, n_coeffs: *const usize,
                          degree_bounds: *const i64, hiding_bounds: *const i64, rng: *mut b2m_rng, out_comm_xy: *mut u64,

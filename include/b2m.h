@@ -40,7 +40,8 @@ enum {
   B2M_ERR_CUDA = 8,
   B2M_ERR_NCCL = 9,
   B2M_ERR_UNSUPPORTED = 10,
-  B2M_ERR_SERIALIZATION = 11            /* [U ark-serialize SerializationError::InvalidData]: an invalid point in a byte stream */
+  B2M_ERR_SERIALIZATION = 11,           /* [U ark-serialize SerializationError::InvalidData]: an invalid point in a byte stream */
+  B2M_ERR_MEMORY_LIMIT = 12             /* the byte model of a key or an index exceeds the device-memory budget (b2m_ctx_set_memory_limit) */
 };
 
 enum { B2M_CURVE_BLS12_381 = 0, B2M_CURVE_BN254 = 1 };
@@ -64,6 +65,17 @@ int b2m_ctx_create(int device, b2m_ctx** out);
 void b2m_ctx_destroy(b2m_ctx* ctx);
 /* Number of kernel launches issued through this context so far. */
 unsigned long long b2m_ctx_launches(const b2m_ctx* ctx);
+/* Device-memory budget for what the library allocates: an SRS created through this context afterwards plans its layout for
+ * min(free device memory, bytes) (0 = no limit: free device memory), and `index` refuses a circuit whose modelled index,
+ * prover and MSM scratch exceed what the limit leaves (B2M_ERR_MEMORY_LIMIT, before anything is allocated).  The library
+ * allocates from the device's default stream-ordered memory pool, which every context on that device in the process shares:
+ * the limit counts the bytes the pool already holds in use, whichever context allocated them. */
+int b2m_ctx_set_memory_limit(b2m_ctx* ctx, size_t bytes);
+/* The device's default memory pool (shared by every context on the device in the process): out[0] = bytes in use,
+ * out[1] = their high-water mark since the previous b2m_ctx_memory call on any context of that device (or since the
+ * process started), out[2] = bytes the pool holds from the device.  Synchronises the context's stream and restarts the
+ * high-water mark for every context of the device. */
+int b2m_ctx_memory(b2m_ctx* ctx, size_t* out);
 /* Multi-GPU MSM (one process per GPU of one node): rank 0 obtains an NCCL unique id (128 bytes), the
  * caller broadcasts it, every rank attaches its context.  From then on every MSM issued through the
  * context is sharded by (base, scalar) chunk across the ranks and the partial sums are exchanged with one
@@ -103,9 +115,26 @@ int b2m_msm_g1(b2m_ctx* ctx, int curve, const uint64_t* bases_xy, const uint64_t
 int b2m_srs_create(b2m_ctx* ctx, int curve, const uint64_t* powers_of_g, size_t n_g,
                    const uint64_t* powers_of_gamma_g, const uint64_t* gamma_indices, size_t n_gamma,
                    int window_bits, b2m_srs** out);
+/* b2m_srs_create with a chosen number of window tables.  window_tables = 0 (what b2m_srs_create passes) keeps all
+ * W = ceil(256 / c) tables whenever the byte model of the largest circuit the key can index fits the context's budget
+ * (b2m_ctx_set_memory_limit), and otherwise keeps the largest T < W (at c <= 16 unless window_bits is set), and caps the
+ * pairs of one MSM bucket pass, that fit; window_tables > 0 forces T (normalised to ceil(W / m) with m = ceil(W / T), the
+ * tables the m bucket sets read; B2M_ERR_INVALID_ARG when m sets of 2^(c-1) buckets exceed 2^24 bucket ids).  Results do not
+ * depend on the layout.  Fails with
+ * B2M_ERR_MEMORY_LIMIT, naming the bytes needed and the budget, when even one table and the smallest pass do not fit, and
+ * with B2M_ERR_UNSUPPORTED for T < W on a multi-GPU context. */
+int b2m_srs_create_layout(b2m_ctx* ctx, int curve, const uint64_t* powers_of_g, size_t n_g,
+                          const uint64_t* powers_of_gamma_g, const uint64_t* gamma_indices, size_t n_gamma,
+                          int window_bits, int window_tables, b2m_srs** out);
 void b2m_srs_destroy(b2m_srs* srs);
 size_t b2m_srs_size(const b2m_srs* srs);
 int b2m_srs_window_bits(const b2m_srs* srs);
+/* Window tables the key keeps (T <= W).  Diagnostic, like b2m_srs_window_bits. */
+int b2m_srs_window_tables(const b2m_srs* srs);
+/* The key's layout and the byte model behind it: out[0] = window bits, [1] = window tables, [2] = pairs per MSM pass
+ * (0: no cap), [3..6] = modelled bytes of the tables, the index and prover of the largest circuit, the MSM scratch, and
+ * their total (with room for the pool's allocation granularity), [7] = the budget the layout was planned for (0 on a multi-GPU context, which does not plan). */
+int b2m_srs_layout(const b2m_srs* srs, size_t* out);
 /* Batched-affine levels the MSMs of this key run before the XYZZ bucket pass (0: none; MSMs with few bucket
  * references skip them regardless).  Diagnostic, like b2m_srs_window_bits. */
 int b2m_srs_affine_levels(const b2m_srs* srs);

@@ -14,6 +14,7 @@ PC_MARLIN_KZG10 = 0
 PC_SONIC_KZG10 = 1
 RNG_CHACHA8, RNG_CHACHA12, RNG_CHACHA20 = 8, 12, 20
 ERR_SERIALIZATION = 11
+ERR_MEMORY_LIMIT = 12
 # per-point causes of B2M_ERR_SERIALIZATION (b2m_g1_decode_ark / b2m_g2_decode_ark)
 POINT_REASONS = {1: "both flag bits set", 2: "x is not below the field modulus", 3: "not on the curve", 4: "not in the prime-order subgroup",
                  5: "y is not below the field modulus"}
@@ -62,6 +63,8 @@ def lib():
         L.b2m_ctx_destroy.restype = None
         L.b2m_ctx_launches.argtypes = [vp]
         L.b2m_ctx_launches.restype = ctypes.c_ulonglong
+        L.b2m_ctx_set_memory_limit.argtypes = [vp, sz]
+        L.b2m_ctx_memory.argtypes = [vp, P(sz)]
         L.b2m_comm_unique_id.argtypes = [vp, sz]
         L.b2m_ctx_attach_comm.argtypes = [vp, vp, sz, ci, ci]
         L.b2m_ctx_profile.argtypes = [vp, ci]
@@ -69,12 +72,15 @@ def lib():
         L.b2m_ntt.argtypes = [vp, ci, vp, ctypes.c_uint, ci, ci]
         L.b2m_msm_g1.argtypes = [vp, ci, vp, vp, sz, vp, P(ci)]
         L.b2m_srs_create.argtypes = [vp, ci, vp, sz, vp, vp, sz, ci, P(vp)]
+        L.b2m_srs_create_layout.argtypes = [vp, ci, vp, sz, vp, vp, sz, ci, ci, P(vp)]
         L.b2m_srs_destroy.argtypes = [vp]
         L.b2m_srs_destroy.restype = None
         L.b2m_srs_size.argtypes = [vp]
         L.b2m_srs_size.restype = sz
         L.b2m_srs_window_bits.argtypes = [vp]
         L.b2m_srs_affine_levels.argtypes = [vp]
+        L.b2m_srs_window_tables.argtypes = [vp]
+        L.b2m_srs_layout.argtypes = [vp, P(sz)]
         L.b2m_srs_msm.argtypes = [vp, sz, vp, sz, vp, P(ci)]
         L.b2m_g1_powers.argtypes = [vp, ci, vp, vp, sz, vp]
         L.b2m_fixed_base_msm.argtypes = [vp, ci, vp, vp, sz, vp]

@@ -21,11 +21,24 @@ PC_IDS = {"marlin_kzg10": _lib.PC_MARLIN_KZG10, "sonic_kzg10": _lib.PC_SONIC_KZG
 
 
 class Context:
-    """One GPU (b2m_ctx)."""
+    """One GPU (b2m_ctx).  memory_limit: device bytes an SRS created through this context plans its window tables and MSM
+    passes for, and `index` checks its circuit against (None: all free device memory).  The library allocates from the
+    device's default memory pool, shared by every Context on that device in the process, so the limit also counts what the
+    other contexts hold."""
 
-    def __init__(self, device=0):
+    def __init__(self, device=0, memory_limit=None):
         self.handle = ctypes.c_void_p()
         _lib.check(_lib.lib().b2m_ctx_create(device, ctypes.byref(self.handle)))
+        if memory_limit:
+            _lib.check(_lib.lib().b2m_ctx_set_memory_limit(self.handle, int(memory_limit)))
+
+    def memory(self):
+        """{"used", "peak", "reserved"}: bytes of the device's default memory pool in use, their high-water mark since the
+        previous call, and bytes the pool holds from the device.  The pool is shared by every Context on the device in the
+        process: the figures include their allocations, and the call restarts the high-water mark for all of them."""
+        out = (ctypes.c_size_t * 3)()
+        _lib.check(_lib.lib().b2m_ctx_memory(self.handle, out))
+        return {"used": int(out[0]), "peak": int(out[1]), "reserved": int(out[2])}
 
     def launches(self):
         return int(_lib.lib().b2m_ctx_launches(self.handle))
@@ -117,6 +130,13 @@ class UniversalSRS:
         self.trapdoor = None  # (beta, gamma) of an insecure test SRS made by universal_setup / srs_from_trapdoor
         self.g2 = None        # (h, beta_h, {index: neg power}) as ark-serialize bytes when loaded from / written to a file
         self.ark = None       # load_ark_srs: the whole file as decoded -- every gamma power and neg_powers_of_h (save_ark)
+
+    def layout(self):
+        """The device layout of the key's MSM tables and the byte model it was chosen by (b2m_srs_layout)."""
+        out = (ctypes.c_size_t * 8)()
+        _lib.check(_lib.lib().b2m_srs_layout(self.handle, out))
+        keys = ("window_bits", "window_tables", "max_pairs", "tables_bytes", "circuit_bytes", "msm_bytes", "model_bytes", "budget")
+        return dict(zip(keys, (int(v) for v in out)))
 
     def save(self, path, degree_bounds=()):
         """Write the SRS as an ark-serialize file (marlin_b200/srsfile.py).  The G2 half -- h, beta h and SonicKZG10's
@@ -406,14 +426,15 @@ class Marlin:
 
     # -- universal_setup ---------------------------------------------------------------------------
     def universal_setup(self, num_constraints, num_variables, num_non_zero, beta, g=None, gamma=7, degree_bounds=(),
-                        window_bits=0):
+                        window_bits=0, window_tables=0):
         """[reference src/lib.rs:79-96] with an explicit trapdoor: an insecure test SRS exactly like the
         reference's `universal_setup(.., test_rng)`, generated on the GPU.  `degree_bounds`: bounds whose
-        shifted gamma powers SonicKZG10 will need (ignored by MarlinKZG10)."""
+        shifted gamma powers SonicKZG10 will need (ignored by MarlinKZG10).  window_bits / window_tables = 0: chosen by the
+        library from the key size and the context's memory budget (b2m_srs_create_layout)."""
         md = max_degree(num_constraints, num_variables, num_non_zero)
-        return self.srs_from_trapdoor(md, beta, g, gamma, degree_bounds, window_bits)
+        return self.srs_from_trapdoor(md, beta, g, gamma, degree_bounds, window_bits, window_tables)
 
-    def srs_from_trapdoor(self, md, beta, g=None, gamma=7, degree_bounds=(), window_bits=0):
+    def srs_from_trapdoor(self, md, beta, g=None, gamma=7, degree_bounds=(), window_bits=0, window_tables=0):
         L = _lib.lib()
         cid = self.curve_id
         lq = _lib.LIMBS[cid][1]
@@ -434,11 +455,11 @@ class Marlin:
         exps = _lib.ints_to_limbs([pow(beta % r, i, r) for i in idx], 4)
         gam = np.zeros((len(idx), 2 * lq), dtype=np.uint64)
         _lib.check(L.b2m_fixed_base_msm(self.ctx.handle, cid, _lib.ptr(gamma_g), _lib.ptr(exps), len(idx), _lib.ptr(gam)))
-        srs = self.srs_from_points(powers, gam, idx, window_bits)
+        srs = self.srs_from_points(powers, gam, idx, window_bits, window_tables)
         srs.trapdoor = (beta % r, gamma % r)
         return srs
 
-    def load_srs(self, path, window_bits=0):
+    def load_srs(self, path, window_bits=0, window_tables=0):
         """Load an SRS file (marlin_b200/srsfile.py layout; `deserialize_unchecked` semantics: no subgroup check)."""
         from . import srsfile
         L = _lib.lib()
@@ -455,11 +476,11 @@ class Marlin:
         graw = np.frombuffer(b"".join(d["gamma"][k] for k in idx), dtype=np.uint8)
         gam = np.zeros((len(idx), 2 * lq), dtype=np.uint64)
         _lib.check(L.b2m_g1_from_uncompressed(self.ctx.handle, self.curve_id, _lib.ptr(np.ascontiguousarray(graw)), len(idx), _lib.ptr(gam)))
-        srs = self.srs_from_points(powers, gam, idx, window_bits)
+        srs = self.srs_from_points(powers, gam, idx, window_bits, window_tables)
         srs.g2 = (d["h"], d["beta_h"], d["neg_powers"])
         return srs
 
-    def load_ark_srs(self, path, compressed=True, degree_bounds=(), window_bits=0):
+    def load_ark_srs(self, path, compressed=True, degree_bounds=(), window_bits=0, window_tables=0):
         """Load a raw arkworks `kzg10::UniversalParams` file, as `UniversalParams::serialize` (compressed=True) or
         `serialize_uncompressed` wrote it, with `deserialize` semantics: every point is decoded and validated on the GPU (flags,
         coordinates below p, on the curve, in the prime-order subgroup), and the first invalid one raises B2MError
@@ -517,21 +538,22 @@ class Marlin:
         missing = [k for k, p in zip(idx, pos) if p >= len(gkeys) or int(gkeys[p]) != k]
         if missing:
             raise ValueError(f"{path}: powers_of_gamma_g holds no entry for the indices {missing}")
-        srs = self.srs_from_points(powers, gamma_all[pos], idx, window_bits)
+        srs = self.srs_from_points(powers, gamma_all[pos], idx, window_bits, window_tables)
         h, beta_h, neg = g2_out[0], g2_out[1], np.ascontiguousarray(g2_out[2:])
         srs.g2 = (h.tobytes(), beta_h.tobytes(), srsfile.G2Points(nkeys, neg))
         srs.ark = {"gamma_keys": gkeys, "gamma_limbs": gamma_all, "h": h, "beta_h": beta_h, "neg_keys": nkeys, "neg": neg}
         return srs
 
-    def srs_from_points(self, powers_limbs, gamma_limbs, gamma_indices, window_bits=0):
-        """Upload an existing SRS (affine Montgomery limbs, as ark-ff stores them)."""
+    def srs_from_points(self, powers_limbs, gamma_limbs, gamma_indices, window_bits=0, window_tables=0):
+        """Upload an existing SRS (affine Montgomery limbs, as ark-ff stores them).  window_tables > 0 keeps that many window
+        tables instead of the planned number (the proof bytes do not depend on it)."""
         L = _lib.lib()
         h = ctypes.c_void_p()
         gi = np.asarray(gamma_indices, dtype=np.uint64)
         powers_limbs = np.ascontiguousarray(powers_limbs)
         gamma_limbs = np.ascontiguousarray(gamma_limbs)
-        _lib.check(L.b2m_srs_create(self.ctx.handle, self.curve_id, _lib.ptr(powers_limbs), len(powers_limbs), _lib.ptr(gamma_limbs),
-                                    _lib.ptr(gi), len(gi), window_bits, ctypes.byref(h)))
+        _lib.check(L.b2m_srs_create_layout(self.ctx.handle, self.curve_id, _lib.ptr(powers_limbs), len(powers_limbs), _lib.ptr(gamma_limbs),
+                                           _lib.ptr(gi), len(gi), window_bits, window_tables, ctypes.byref(h)))
         return UniversalSRS(self.ctx, self.curve_id, h, len(powers_limbs) - 1, powers_limbs, gamma_limbs, [int(i) for i in gi])
 
     # -- PC::trim (Level 1) ---------------------------------------------------------------------------------

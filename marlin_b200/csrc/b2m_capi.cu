@@ -38,6 +38,27 @@ void b2m_ctx_destroy(b2m_ctx* ctx) {
 
 unsigned long long b2m_ctx_launches(const b2m_ctx* ctx) { return ctx ? ctx->cx.launches : 0; }
 
+int b2m_ctx_set_memory_limit(b2m_ctx* ctx, size_t bytes) {
+  return guard([&] {
+    B2M_REQUIRE(ctx != nullptr, B2M_ERR_INVALID_ARG, "null argument");
+    ctx->cx.memory_limit = bytes;
+  });
+}
+
+int b2m_ctx_memory(b2m_ctx* ctx, size_t* out) {
+  return guard([&] {
+    B2M_REQUIRE(ctx && out, B2M_ERR_INVALID_ARG, "null argument");
+    Ctx& cx = ctx->cx;
+    cx.use();
+    cx.sync();
+    out[0] = (size_t)cx.pool_attr(cudaMemPoolAttrUsedMemCurrent);
+    out[1] = (size_t)cx.pool_attr(cudaMemPoolAttrUsedMemHigh);
+    out[2] = (size_t)cx.pool_attr(cudaMemPoolAttrReservedMemCurrent);
+    uint64_t zero = 0;  // the high-water mark restarts from what is in use now
+    B2M_CUDA(cudaMemPoolSetAttribute(cx.pool, cudaMemPoolAttrUsedMemHigh, &zero));
+  });
+}
+
 int b2m_comm_unique_id(uint8_t* id, size_t cap) {
   return guard([&] {
     B2M_REQUIRE(id && cap >= sizeof(ncclUniqueId), B2M_ERR_INVALID_ARG, "id buffer must hold %zu bytes", sizeof(ncclUniqueId));
@@ -91,15 +112,21 @@ int b2m_ntt(b2m_ctx* ctx, int curve, uint64_t* data, unsigned log_n, int inverse
   });
 }
 
-int b2m_srs_create(b2m_ctx* ctx, int curve, const uint64_t* powers_of_g, size_t n_g, const uint64_t* powers_of_gamma_g,
-                   const uint64_t* gamma_indices, size_t n_gamma, int window_bits, b2m_srs** out) {
+int b2m_srs_create_layout(b2m_ctx* ctx, int curve, const uint64_t* powers_of_g, size_t n_g, const uint64_t* powers_of_gamma_g,
+                          const uint64_t* gamma_indices, size_t n_gamma, int window_bits, int window_tables, b2m_srs** out) {
   return guard([&] {
     B2M_REQUIRE(ctx && powers_of_g && out, B2M_ERR_INVALID_ARG, "null argument");
     B2M_REQUIRE(curve == B2M_CURVE_BLS12_381 || curve == B2M_CURVE_BN254, B2M_ERR_INVALID_ARG, "unknown curve id");
+    B2M_REQUIRE(window_tables >= 0, B2M_ERR_INVALID_ARG, "window_tables %d < 0", window_tables);
     ctx->cx.use();
-    *out = new b2m_srs(ctx, curve, powers_of_g, n_g, powers_of_gamma_g, gamma_indices, n_gamma, window_bits);
+    *out = new b2m_srs(ctx, curve, powers_of_g, n_g, powers_of_gamma_g, gamma_indices, n_gamma, window_bits, window_tables);
     ctx->children++;
   });
+}
+
+int b2m_srs_create(b2m_ctx* ctx, int curve, const uint64_t* powers_of_g, size_t n_g, const uint64_t* powers_of_gamma_g,
+                   const uint64_t* gamma_indices, size_t n_gamma, int window_bits, b2m_srs** out) {
+  return b2m_srs_create_layout(ctx, curve, powers_of_g, n_g, powers_of_gamma_g, gamma_indices, n_gamma, window_bits, 0, out);
 }
 
 void b2m_srs_destroy(b2m_srs* srs) {
@@ -114,6 +141,16 @@ void b2m_srs_destroy(b2m_srs* srs) {
 size_t b2m_srs_size(const b2m_srs* srs) { return srs ? srs->n_g : 0; }
 int b2m_srs_window_bits(const b2m_srs* srs) { return srs ? srs->window_bits() : 0; }
 int b2m_srs_affine_levels(const b2m_srs* srs) { return srs ? srs->affine_levels() : 0; }
+int b2m_srs_window_tables(const b2m_srs* srs) { return srs ? srs->window_tables() : 0; }
+int b2m_srs_layout(const b2m_srs* srs, size_t* out) {
+  return guard([&] {
+    B2M_REQUIRE(srs && out, B2M_ERR_INVALID_ARG, "null argument");
+    const MsmBytes& b = srs->layout.bytes;
+    const size_t v[8] = {(size_t)srs->window_bits(), (size_t)srs->window_tables(), srs->layout.max_pairs, b.tables, b.circuit, b.msm, b.total(),
+                         srs->budget};
+    memcpy(out, v, sizeof(v));
+  });
+}
 
 int b2m_srs_msm(b2m_srs* srs, size_t base_off, const uint64_t* scalars, size_t n, uint64_t* out_xy, int* out_is_inf) {
   return guard([&] {

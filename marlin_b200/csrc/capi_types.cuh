@@ -63,21 +63,84 @@ struct b2m_srs {
     throw b2m::Error(B2M_ERR_INVALID_ARG, b2m::fmt("the SRS holds no power %llu of gamma*G", (unsigned long long)i));
   }
 
+  b2m::MsmKeyShape shape;   // what the byte model knows of this key
+  b2m::MsmLayout layout;    // the planned layout and the model's figures for it
+  size_t budget = 0;        // pool bytes available when the key was created
+
   b2m_srs(b2m_ctx* c, int curve_, const uint64_t* g, size_t ng, const uint64_t* gamma, const uint64_t* gidx, size_t ngamma,
-          int window_bits)
+          int window_bits, int window_tables)
       : ctx(c), curve(curve_), n_g(ng), n_gamma(ngamma) {
     using namespace b2m;
     for (size_t k = 0; k < ngamma; k++) gamma_idx.push_back(gidx ? gidx[k] : k);
     if (curve == B2M_CURVE_BLS12_381) {
+      plan<FrBls, FqBls>(window_bits, window_tables);
       bls.reset(new Msm<FrBls, FqBls>(c->cx, reinterpret_cast<const Affine<FqBls>*>(g), ng, reinterpret_cast<const Affine<FqBls>*>(gamma), ngamma,
-                                      window_bits));
+                                      layout.c, false, layout.T, layout.max_pairs));
     } else {
+      plan<FrBn, FqBn>(window_bits, window_tables);
       bn.reset(new Msm<FrBn, FqBn>(c->cx, reinterpret_cast<const Affine<FqBn>*>(g), ng, reinterpret_cast<const Affine<FqBn>*>(gamma), ngamma,
-                                  window_bits));
+                                  layout.c, false, layout.T, layout.max_pairs));
     }
     c->cx.sync();
   }
+
+  // Layout of the key (msm_layout.hpp): all W window tables whenever the byte model of the largest circuit the key can index
+  // fits min(free device memory, the context's memory limit); else the largest T < W and MSM pass cap that fit; else
+  // B2M_ERR_MEMORY_LIMIT before anything is allocated.  window_tables > 0 (or B2M_MSM_TABLES) forces T, B2M_MSM_MAX_PAIRS the
+  // pass cap (tests).  A multi-GPU context keeps its tables sharded by rank instead: the full layout only.
+  template <class Fr, class Fq>
+  void plan(int window_bits, int window_tables) {
+    using namespace b2m;
+    Ctx& cx = ctx->cx;
+    int forced_T = window_tables;
+    size_t forced_cap = 0;
+    if (const char* e = getenv("B2M_MSM_TABLES")) forced_T = atoi(e);
+    if (const char* e = getenv("B2M_MSM_MAX_PAIRS")) forced_cap = (size_t)atoll(e);
+    B2M_REQUIRE(window_bits == 0 || (window_bits >= MSM_MIN_WINDOW && window_bits <= 24), B2M_ERR_INVALID_ARG, "window bits %d out of range [%d, 24]",
+                window_bits, MSM_MIN_WINDOW);
+    B2M_REQUIRE(n_g >= 1, B2M_ERR_INVALID_ARG, "SRS size %zu out of range", n_g);
+    shape = MsmKeyShape{n_g, n_gamma, Fr::Params::BITS, sizeof(Fq), Fq::N > 8 ? 3 : 0};
+    if (const char* e = getenv("B2M_MSM_AFFINE_LEVELS")) shape.affine_levels = atoi(e);
+    const int c_full = window_bits > 0 ? window_bits : Msm<Fr, Fq>::pick_window(n_g / (size_t)(cx.world > 1 ? cx.world : 1));
+    if (cx.world > 1) {  // (Msm rejects a forced reduction with B2M_ERR_UNSUPPORTED)
+      layout.c = c_full;
+      layout.T = forced_T;
+      layout.max_pairs = forced_cap;
+      return;
+    }
+    const int c_reduced = window_bits > 0 ? window_bits : std::min(c_full, MSM_REDUCED_WINDOW);
+    const int c_min = window_bits > 0 ? window_bits : MSM_MIN_WINDOW;
+    if (forced_T > 0 && forced_T < msm_windows(shape.fr_bits, c_full)) {  // a forced T the bucket field cannot hold is a bad argument
+      bool fits = false;
+      for (int c = c_reduced; c >= c_min && !fits; c--) fits = msm_sets_fit(c, msm_sets(msm_windows(shape.fr_bits, c), forced_T));
+      const int m = msm_sets(msm_windows(shape.fr_bits, c_reduced), forced_T);
+      B2M_REQUIRE(fits, B2M_ERR_INVALID_ARG, "%d window table(s) at c = %d need %d bucket sets of 2^%d buckets, more than the 2^%d bucket ids",
+                  forced_T, c_reduced, m, c_reduced - 1, MSM_BKT_BITS);
+    }
+    budget = cx.memory_budget();
+    layout = msm_plan_layout(shape, c_full, c_reduced, c_min, budget, forced_T, forced_cap);
+    const MsmBytes& b = layout.bytes;
+    B2M_REQUIRE(layout.T > 0, B2M_ERR_MEMORY_LIMIT,
+                "an SRS of %zu powers needs %zu bytes (window tables %zu, index and prover %zu, MSM scratch %zu at %d table(s), c = %d, "
+                "%zu-pair passes) for the largest circuit it can index; the device-memory budget is %zu bytes",
+                n_g, b.total(), b.tables, b.circuit, b.msm, layout.T ? layout.T : 1, layout.c, layout.max_pairs, budget);
+  }
+
+  // `index` of a circuit with |K| = K, |H| = H on this key: with a memory limit set, refuse before allocating when the model
+  // of its index, prover and MSM scratch (sized for this circuit's largest MSM, not the whole key) exceeds what the limit
+  // leaves.
+  void require_fits(size_t K, size_t H) const {
+    using namespace b2m;
+    Ctx& cx = ctx->cx;
+    if (!cx.memory_limit || cx.world > 1) return;
+    const MsmBytes b = msm_model_bytes(shape, layout.c, layout.T, layout.max_pairs, K, H);
+    const size_t avail = cx.memory_budget();
+    B2M_REQUIRE(b.circuit + b.msm <= avail, B2M_ERR_MEMORY_LIMIT,
+                "an index of |K| = %zu, |H| = %zu needs %zu bytes (index and prover %zu, MSM scratch %zu); the device-memory budget leaves %zu bytes",
+                K, H, b.circuit + b.msm, b.circuit, b.msm, avail);
+  }
   int window_bits() const { return bls ? bls->c : bn->c; }
+  int window_tables() const { return bls ? bls->T : bn->T; }
   int affine_levels() const { return bls ? bls->affine_levels : bn->affine_levels; }
   size_t affine_min_refs() const { return bls ? bls->affine_min_refs : bn->affine_min_refs; }
 };

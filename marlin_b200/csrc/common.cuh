@@ -3,7 +3,9 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdarg>
+#include <cstdint>
 #include <cstdio>
 #include <stdexcept>
 #include <string>
@@ -117,6 +119,25 @@ struct Ctx {
   }
   void use() const { cudaSetDevice(device); }
   void sync() { B2M_CUDA(cudaStreamSynchronize(stream)); }
+
+  // b2m_ctx_set_memory_limit: pool bytes the SRS layout planner and the index check may count on (0: no limit)
+  size_t memory_limit = 0;
+  uint64_t pool_attr(cudaMemPoolAttr a) const {
+    uint64_t v = 0;
+    B2M_CUDA(cudaMemPoolGetAttribute(pool, a, &v));
+    return v;
+  }
+  // Bytes the library may still take from its pool: free device memory plus what the pool holds unused, and at most the
+  // limit minus what the pool already holds in use.
+  size_t memory_budget() {
+    sync();
+    size_t free_b = 0, total_b = 0;
+    B2M_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    const uint64_t reserved = pool_attr(cudaMemPoolAttrReservedMemCurrent), used = pool_attr(cudaMemPoolAttrUsedMemCurrent);
+    size_t avail = free_b + (size_t)(reserved - used);
+    if (memory_limit) avail = std::min<size_t>(avail, memory_limit > used ? memory_limit - (size_t)used : 0);
+    return avail;
+  }
   void* alloc_bytes(size_t n) {
     void* p = nullptr;
     if (n == 0) n = 16;

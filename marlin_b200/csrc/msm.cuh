@@ -21,18 +21,17 @@
 //   5. reduce:      sum_b (b+1) B_b through row / column sums of the 2-D bucket view, bit planes, one Horner fold
 // The result is a unique group element, compared with the oracle in affine form.
 #pragma once
+// A key that cannot hold all W tables keeps T < W of them and splits its bucket problem into m = ceil(W / T) bucket sets, and
+// long MSMs can run as several bucket passes of at most max_pairs pairs (msm_layout.hpp).
 #include "common.cuh"
 #include "curve.cuh"
+#include "msm_layout.hpp"
 
 namespace b2m {
 
-constexpr int MSM_MIN_WINDOW = 8;  // at most ceil(256 / 8) = 32 windows
-constexpr int MSM_BKT_BITS = 24;  // a sorted reference is {table index | sign << 31, bucket | window << 24}
 constexpr uint32_t MSM_BKT_MASK = (1u << MSM_BKT_BITS) - 1;
 constexpr uint32_t MSM_NO_DIGIT = 0xffffffffu;
-constexpr int MSM_MAX_BATCH = 8;   // MSMs per run_batch call
 constexpr int MSM_MAX_AFFINE_LEVELS = 6;
-constexpr size_t MSM_AFFINE_MIN_REFS = (size_t)1 << 23;  // MSMs with fewer bucket references skip the batched-affine levels (latency-bound below)
 
 template <class Fr, class Fq>
 struct MsmJob {
@@ -59,6 +58,8 @@ struct Msm {
   size_t n_extra = 0;  // further fixed bases (powers_of_gamma_g) appended after them
   size_t stride = 0;   // n_srs + n_extra: entries per window table
   int c = 0, W = 0;
+  int T = 0, m = 1;        // window tables kept, bucket sets per MSM (m = ceil(W / T); T = W, m = 1: the full layout)
+  size_t max_pairs = 0;    // pairs per bucket pass (0: one pass per MSM)
   // batched-affine levels run before the XYZZ bucket pass (msm_affine.cuh); override: B2M_MSM_AFFINE_LEVELS.
   // Off for a 254-bit Fq: its multiplications are so cheap that the levels' extra memory traffic costs more
   // than the saved multiplications.
@@ -73,13 +74,14 @@ struct Msm {
   int affine_T = 64;        // additions per thread (chain) at level 0; B2M_MSM_AFFINE_T sets both
   int affine_T_upper = 32;  // ... at levels >= 1; B2M_MSM_AFFINE_T_UPPER
   int acc_ctas_per_sm = 3;  // resident CTAs of msm_accumulate_kernel per SM (occupancy query)
-  DBuf<Affine<Fq>> tables;  // [W][stride]:  tables[w * stride + k] = 2^(c*w) * P_(k * world + rank)
+  DBuf<Affine<Fq>> tables;  // [T][stride]:  tables[j * stride + k] = 2^(c*m*j) * P_(k * world + rank)
 
   static int pick_window(size_t n);
   // Upload the powers and build the window tables (key-load time).  powers_on_device: `powers` is a device array (the
-  // verifier's decoded proof points), copied on the device; single-GPU contexts only.
+  // verifier's decoded proof points), copied on the device; single-GPU contexts only.  n_tables (0: all W) and max_pairs
+  // (0: no cap) choose a reduced layout; multi-GPU contexts take the full one only.
   Msm(Ctx& cx, const Affine<Fq>* powers, size_t n, const Affine<Fq>* host_extra, size_t n_extra_bases, int window_bits,
-      bool powers_on_device = false);
+      bool powers_on_device = false, int n_tables = 0, size_t max_pairs = 0);
 
   // sum_i scalars[i] * powers[base_off + i] (+ the `extra` XYZZ terms) -> out_xyzz / out_affine on
   // the device.  `scalars` is a device array, Montgomery form if mont, canonical otherwise.
@@ -88,6 +90,8 @@ struct Msm {
   // Several MSMs at once (the commitments of one prover round): bucket passes back to back, then ONE
   // batched log-depth reduction, so its latency is paid per round instead of per MSM.
   void run_batch(const MsmJob<Fr, Fq>* jobs, int nj);
+  // One bucket pass per job (run_batch splits jobs longer than max_pairs into several of these).
+  void run_pass(const MsmJob<Fr, Fq>* jobs, int nj);
   // Level-0 ABI bodies (include/b2m.h): host scalars in, host affine point out.
   void run_host(size_t base_off, const uint64_t* scalars, size_t n, uint64_t* out_xy, int* out_is_inf);
   // powers_of_g[i] (affine Montgomery limbs) back to the host: window-0 table entry, from the GPU that holds it

@@ -71,11 +71,11 @@ __global__ void msm_take_residue_kernel(const Affine<Fq>* all, size_t n_loc, int
 }
 
 // ---- 1. digits ----------------------------------------------------------------------------
-// digits[w * nt + i] = (|d| - 1) | sign << 31, or MSM_NO_DIGIT for d == 0; hist[|d| - 1]++.
+// digits[w * nt + i] = (w % m) 2^(c-1) + (|d| - 1) | sign << 31, or MSM_NO_DIGIT for d == 0; hist[that bucket]++.
 // Scalars come in two groups: i < n from `scalars` (the polynomial), the rest from `scalars2`
-// (the few blinding coefficients that multiply the gamma powers), nt = n + n2.
+// (the few blinding coefficients that multiply the gamma powers), nt = n + n2.  m = 1: one bucket set (all W tables).
 template <class Fr>
-__global__ void msm_digits_kernel(const Fr* scalars, size_t sstride, const Fr* scalars2, bool MONT, size_t n, size_t nt, int c, int W,
+__global__ void msm_digits_kernel(const Fr* scalars, size_t sstride, const Fr* scalars2, bool MONT, size_t n, size_t nt, int c, int W, int m,
                                   uint32_t* digits, uint32_t* hist) {
   size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   if (i >= nt) return;
@@ -93,14 +93,15 @@ __global__ void msm_digits_kernel(const Fr* scalars, size_t sstride, const Fr* s
       raw &= (1u << c) - 1;
     }
     uint32_t v = raw + carry;
+    const uint32_t set_off = (uint32_t)(w % m) * half;
     uint32_t out;
     if (v > half) {
-      uint32_t mag = (1u << c) - v;  // d = v - 2^c < 0
+      uint32_t mag = (1u << c) - v;  // d = v - 2^c < 0, or d = 0 when v = 2^c (raw all ones plus a carry)
       carry = 1;
-      out = (mag - 1) | 0x80000000u;
+      out = mag ? (set_off + mag - 1) | 0x80000000u : MSM_NO_DIGIT;
     } else {
       carry = 0;
-      out = v ? (v - 1) : MSM_NO_DIGIT;
+      out = v ? (set_off + v - 1) : MSM_NO_DIGIT;
     }
     digits[(size_t)w * nt + i] = out;
     if (out != MSM_NO_DIGIT) atomicAdd(hist + (out & 0x7fffffffu), 1u);
@@ -110,8 +111,8 @@ __global__ void msm_digits_kernel(const Fr* scalars, size_t sstride, const Fr* s
 // ---- 2. exclusive scan of u32: scan.cuh -------------------------------------------------------
 
 // ---- 3. scatter -------------------------------------------------------------------------------
-// Counting sort by bucket: sorted[pos] = {(absolute table index) | sign << 31, bucket | window << 24}.
-static __global__ void msm_scatter_kernel(const uint32_t* digits, size_t n, size_t nt, size_t base_off, size_t idx2, int W,
+// Counting sort by bucket: sorted[pos] = {(absolute table index) | sign << 31, bucket | table << 24}, table = window / m.
+static __global__ void msm_scatter_kernel(const uint32_t* digits, size_t n, size_t nt, size_t base_off, size_t idx2, int W, int m,
                                           uint32_t* cursor, uint2* sorted) {
   size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   if (i >= nt) return;
@@ -121,7 +122,7 @@ static __global__ void msm_scatter_kernel(const uint32_t* digits, size_t n, size
     if (d == MSM_NO_DIGIT) continue;
     uint32_t bkt = d & 0x7fffffffu;
     uint32_t pos = atomicAdd(cursor + bkt, 1u);
-    sorted[pos] = make_uint2(abs_idx | (d & 0x80000000u), bkt | ((uint32_t)w << MSM_BKT_BITS));  // one 8-byte scattered store
+    sorted[pos] = make_uint2(abs_idx | (d & 0x80000000u), bkt | ((uint32_t)(w / m) << MSM_BKT_BITS));  // one 8-byte scattered store
   }
 }
 
@@ -528,7 +529,53 @@ __global__ void __launch_bounds__(64) msm_finish_kernel(const XYZZ<Fq>* rplanes,
   }
 }
 
+// Reduced-table keys (m > 1 bucket sets per MSM): sums[g] = sum_b (b + 1) B_b of bucket set g (g = job * m + set), as
+// msm_finish_kernel folds it, one block per set.
+template <class Fq>
+__global__ void __launch_bounds__(64) msm_set_sum_kernel(const XYZZ<Fq>* rplanes, int rbits, const XYZZ<Fq>* cplanes, int cbits, XYZZ<Fq>* sums) {
+  __shared__ uint4 sm_raw[2 * sizeof(XYZZ<Fq>) / 16];
+  XYZZ<Fq>* sm = reinterpret_cast<XYZZ<Fq>*>(sm_raw);
+  const size_t g = blockIdx.x;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0) {
+    XYZZ<Fq> acc = XYZZ<Fq>::inf();
+    const XYZZ<Fq>* pl = warp == 0 ? rplanes + g * (rbits + 1) : cplanes + g * (cbits + 1);
+    const int nb = warp == 0 ? rbits : cbits;
+    for (int k = nb - 1; k >= 0; k--) {
+      g1_dbl(acc);
+      g1_add(acc, ld_words(pl + k));
+    }
+    if (warp == 0) {
+      for (int k = 0; k < cbits; k++) g1_dbl(acc);
+      g1_add(acc, ld_words(pl + rbits));
+    }
+    sm[warp] = acc;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    XYZZ<Fq> total = sm[0];
+    g1_add(total, sm[1]);
+    st_words(sums + g, total);
+  }
+}
+// ... then per job: result = sum_k 2^(c k) sums[job * m + k] (Horner, c (m - 1) doublings) + extras.
+template <class Fq>
+__global__ void __launch_bounds__(32) msm_sets_finish_kernel(const XYZZ<Fq>* sums, int m, int c, MsmFinishJobs jobs) {
+  const int j = blockIdx.x;
+  if (threadIdx.x != 0) return;
+  XYZZ<Fq> total = ld_words(sums + (size_t)j * m + (m - 1));
+  for (int k = m - 2; k >= 0; k--) {
+    for (int i = 0; i < c; i++) g1_dbl(total);
+    g1_add(total, ld_words(sums + (size_t)j * m + k));
+  }
+  const XYZZ<Fq>* extra = reinterpret_cast<const XYZZ<Fq>*>(jobs.j[j].extra);
+  for (int i = 0; i < jobs.j[j].n_extra; i++) g1_add(total, ld_words(extra + i));
+  if (jobs.j[j].out_xyzz) st_words(reinterpret_cast<XYZZ<Fq>*>(jobs.j[j].out_xyzz), total);
+  if (jobs.j[j].out_affine) st_words(reinterpret_cast<Affine<Fq>*>(jobs.j[j].out_affine), g1_to_affine(total));
+}
+
 // Multi-GPU: out_j = sum_r partial[r][j] + extras (every rank computes the same sum in the same order).
+// Passes (run_batch): the same with r = pass.
 template <class Fq>
 __global__ void __launch_bounds__(32) msm_combine_kernel(const XYZZ<Fq>* all, int world, int nj, MsmFinishJobs jobs) {
   const int j = blockIdx.x;
@@ -647,8 +694,8 @@ int Msm<Fr, Fq>::pick_window(size_t n) {
 
 template <class Fr, class Fq>
 Msm<Fr, Fq>::Msm(Ctx& cx, const Affine<Fq>* host_powers, size_t n, const Affine<Fq>* host_extra, size_t n_extra_bases, int window_bits,
-                 bool powers_on_device)
-    : ctx(&cx), n_extra(n_extra_bases), n_srs_global(n) {
+                 bool powers_on_device, int n_tables, size_t max_pairs_)
+    : ctx(&cx), n_extra(n_extra_bases), n_srs_global(n), max_pairs(max_pairs_) {
   B2M_REQUIRE(!powers_on_device || cx.world <= 1, B2M_ERR_UNSUPPORTED, "device-resident bases on a multi-GPU context");
   // Multi-GPU: GPU r keeps only the powers i = r (mod world) -- every contiguous slice of the key, whatever its
   // offset and length, then splits evenly over the GPUs, and table memory and build time drop by `world`.
@@ -661,7 +708,13 @@ Msm<Fr, Fq>::Msm(Ctx& cx, const Affine<Fq>* host_powers, size_t n, const Affine<
   B2M_REQUIRE(c >= MSM_MIN_WINDOW && c <= 24, B2M_ERR_INVALID_ARG, "window bits %d out of range [%d, 24]", c, MSM_MIN_WINDOW);
   W = (Fr::Params::BITS + 1 + c - 1) / c;
   B2M_REQUIRE(W <= 32, B2M_ERR_INVALID_ARG, "too many windows (%d)", W);
-  tables = DBuf<Affine<Fq>>(cx, (size_t)W * stride);
+  T = n_tables > 0 && n_tables < W ? msm_tables_used(W, n_tables) : W;  // (no table that no window reads)
+  B2M_REQUIRE((T == W && max_pairs == 0) || tab_world == 1, B2M_ERR_UNSUPPORTED,
+              "reduced window tables (%d of %d) or an MSM pass cap (%zu pairs) on a multi-GPU context", T, W, max_pairs);
+  m = msm_sets(W, T);
+  B2M_REQUIRE(msm_sets_fit(c, m), B2M_ERR_INVALID_ARG, "%d window tables at c = %d: %d bucket sets of 2^%d buckets exceed the 2^%d bucket ids", T, c,
+              m, c - 1, MSM_BKT_BITS);
+  tables = DBuf<Affine<Fq>>(cx, (size_t)T * stride);
   if (powers_on_device) {
     B2M_CUDA(cudaMemcpyAsync(tables.p, host_powers, n * sizeof(Affine<Fq>), cudaMemcpyDeviceToDevice, cx.stream));
   } else if (tab_world == 1) {
@@ -675,7 +728,8 @@ Msm<Fr, Fq>::Msm(Ctx& cx, const Affine<Fq>* host_powers, size_t n, const Affine<
   }
   if (n_extra) B2M_CUDA(cudaMemcpyAsync(tables.p + n_srs, host_extra, n_extra * sizeof(Affine<Fq>), cudaMemcpyHostToDevice, cx.stream));
   if (stride) {  // (a rank can own none of a tiny key's powers)
-    msm_precompute_kernel<Fq><<<div_up(stride, 128), 128, 0, cx.stream>>>(tables.p, stride, c, W);
+    // table j = 2^(c m j) P: c m doublings between tables (m = 1: one window apart)
+    msm_precompute_kernel<Fq><<<div_up(stride, 128), 128, 0, cx.stream>>>(tables.p, stride, c * m, T);
     B2M_CHECK_LAUNCH();
     cx.launches++;
   }
@@ -705,8 +759,50 @@ void Msm<Fr, Fq>::run(const Fr* scalars, bool mont, size_t n, size_t base_off, c
   run_batch(&job, 1);
 }
 
+// Jobs longer than max_pairs run as passes over consecutive slices of at most max_pairs pairs: pass p of every job is an
+// ordinary bucket pass into partial[p][job] (the blinding group rides with pass 0), and one kernel adds the partial sums
+// and the extra terms.  The sort and level scratch is then sized for max_pairs pairs instead of the whole key.
 template <class Fr, class Fq>
-void Msm<Fr, Fq>::run_batch(const MsmJob<Fr, Fq>* jobs_in, int nj) {
+void Msm<Fr, Fq>::run_batch(const MsmJob<Fr, Fq>* jobs, int nj) {
+  B2M_REQUIRE(nj >= 1 && nj <= MSM_MAX_BATCH, B2M_ERR_INVALID_ARG, "MSM batch of %d jobs", nj);
+  size_t passes = 1;
+  for (int j = 0; j < nj && max_pairs; j++) passes = std::max(passes, (jobs[j].n + max_pairs - 1) / max_pairs);
+  if (passes == 1) {
+    run_pass(jobs, nj);
+    return;
+  }
+  Ctx& cx = *ctx;
+  for (int j = 0; j < nj; j++)
+    B2M_REQUIRE(jobs[j].base_off + jobs[j].n <= n_srs_global, B2M_ERR_DEGREE_TOO_LARGE, "MSM slice [%zu, %zu) exceeds the SRS (%zu powers)",
+                jobs[j].base_off, jobs[j].base_off + jobs[j].n, n_srs_global);
+  DBuf<XYZZ<Fq>> partial(cx, passes * nj);
+  partial.zero();  // (a job with fewer passes leaves its later slots at infinity)
+  for (size_t p = 0; p < passes; p++) {
+    MsmJob<Fr, Fq> sub[MSM_MAX_BATCH];
+    int ns = 0;
+    const size_t at = p * max_pairs;
+    for (int j = 0; j < nj; j++) {
+      if (p > 0 && at >= jobs[j].n) continue;
+      MsmJob<Fr, Fq> s = jobs[j];
+      s.n = at < jobs[j].n ? std::min(max_pairs, jobs[j].n - at) : 0;
+      s.scalars = jobs[j].scalars + at * jobs[j].scalar_stride;
+      s.base_off = jobs[j].base_off + at;
+      if (p > 0) { s.scalars2 = nullptr; s.n2 = 0; }
+      s.extra = nullptr; s.n_extra = 0;
+      s.out_xyzz = partial.p + p * nj + j; s.out_affine = nullptr;
+      sub[ns++] = s;
+    }
+    run_pass(sub, ns);
+  }
+  MsmFinishJobs fj;
+  for (int j = 0; j < nj; j++) fj.j[j] = MsmFinishJob{jobs[j].extra, jobs[j].n_extra, jobs[j].out_xyzz, jobs[j].out_affine};
+  msm_combine_kernel<Fq><<<nj, 32, 0, cx.stream>>>(partial.p, (int)passes, nj, fj);
+  B2M_CHECK_LAUNCH();
+  cx.launches++;
+}
+
+template <class Fr, class Fq>
+void Msm<Fr, Fq>::run_pass(const MsmJob<Fr, Fq>* jobs_in, int nj) {
   Ctx& cx = *ctx;
   B2M_REQUIRE(nj >= 1 && nj <= MSM_MAX_BATCH, B2M_ERR_INVALID_ARG, "MSM batch of %d jobs", nj);
   // Multi-GPU (comm.cuh): the prover runs replicated, so every rank holds the full scalar vectors, but only the
@@ -771,21 +867,33 @@ void Msm<Fr, Fq>::run_batch(const MsmJob<Fr, Fq>* jobs_in, int nj) {
     return;
   }
   const uint32_t B = 1u << (c - 1);
+  const uint32_t NB = (uint32_t)m * B;  // buckets per MSM: m sets of B (set k takes the windows w = k mod m)
+  const size_t G = (size_t)nj * m;      // bucket sets of the batch, each reduced on its own
   const int cbits = (c - 1 + 1) / 2, rbits = (c - 1) - cbits;  // L = 2^cbits columns, R = 2^rbits rows
   const size_t L = (size_t)1 << cbits, R = (size_t)1 << rbits;
-  DBuf<XYZZ<Fq>> buckets(cx, (size_t)nj * B);
+  DBuf<XYZZ<Fq>> buckets(cx, (size_t)nj * NB);
   {
     // Software pipeline over the jobs: the counting sort of job j + 1 (memory / atomic bound, ~40 registers per
     // thread) runs on the side stream while job j's bucket pass (integer-ALU bound, 2 CTAs/SM) runs on the main
     // stream; sort buffers are double-buffered and the two streams are chained with events.
     const size_t max_refs = (size_t)W * max_n;
-    const size_t max_threads = (max_refs + MSM_Q_MIN - 1) / MSM_Q_MIN + 256;  // launches round up to whole blocks
+    // batched-affine levels (msm_affine.cuh): level l has at most bound[l] points.  bound[l] exceeds bound[l - 1] when there
+    // are more buckets than references (forced levels on a small MSM): the buffers take the largest bound of their parity.
+    const int LV = max_refs >= affine_min_refs ? affine_levels : 0;  // (the largest job of the batch decides the buffers)
+    size_t bound[MSM_MAX_AFFINE_LEVELS + 1];
+    bound[0] = max_refs;
+    for (int l = 1; l <= LV; l++) bound[l] = (bound[l - 1] + NB) / 2 + 1;
+    size_t lvl_cap[2] = {0, 0};  // lvl_pts[p] holds the outputs of levels l with (l & 1) == p: bound[l + 1] points
+    for (int l = 0; l < LV; l++) lvl_cap[l & 1] = std::max(lvl_cap[l & 1], bound[l + 1]);
+    // the XYZZ pass reads max_refs references, or bound[LV] points after the levels
+    const size_t acc_refs = LV > 0 ? std::max(max_refs, bound[LV]) : max_refs;
+    const size_t max_threads = (acc_refs + MSM_Q_MIN - 1) / MSM_Q_MIN + 256;  // launches round up to whole blocks
     DBuf<uint32_t> digits[2], hist[2], offsets[2], cursor[2];
     DBuf<uint2> sorted[2];
     const int slots = nj > 1 ? 2 : 1;
     for (int s = 0; s < slots; s++) {
-      digits[s] = DBuf<uint32_t>(cx, max_refs); hist[s] = DBuf<uint32_t>(cx, B + 1); offsets[s] = DBuf<uint32_t>(cx, B + 1);
-      cursor[s] = DBuf<uint32_t>(cx, B); sorted[s] = DBuf<uint2>(cx, max_refs);
+      digits[s] = DBuf<uint32_t>(cx, max_refs); hist[s] = DBuf<uint32_t>(cx, NB + 1); offsets[s] = DBuf<uint32_t>(cx, NB + 1);
+      cursor[s] = DBuf<uint32_t>(cx, NB); sorted[s] = DBuf<uint2>(cx, max_refs);
     }
     DBuf<uint32_t> part_bkt(cx, 2 * max_threads), n_long(cx, 4);  // queued long-run entries, second-stage entries, chunk slots, short runs
     const uint32_t long_cap = 1u << 18;
@@ -793,26 +901,21 @@ void Msm<Fr, Fq>::run_batch(const MsmJob<Fr, Fq>* jobs_in, int nj) {
     DBuf<MsmLongRun> long_runs(cx, long_cap), short_runs(cx, long_cap), final_runs(cx, chunk_cap);
     DBuf<XYZZ<Fq>> chunk_pt(cx, chunk_cap);
     DBuf<XYZZ<Fq>> part_pt(cx, 2 * max_threads);
-    // batched-affine levels (msm_affine.cuh): level l has at most bound[l] points
-    const int LV = max_refs >= affine_min_refs ? affine_levels : 0;  // (the largest job of the batch decides the buffers)
-    // the level-0 plan packs (window * stride + index) | sign << 31 into 32 bits (msm_affine.cuh aff_plan_thread)
-    B2M_REQUIRE(LV == 0 || (size_t)W * stride < ((size_t)1 << 31), B2M_ERR_DEGREE_TOO_LARGE,
-                "window tables of %d x %zu entries exceed the 31-bit index of the batched-affine plan", W, stride);
-    size_t bound[MSM_MAX_AFFINE_LEVELS + 1];
-    bound[0] = max_refs;
-    for (int l = 1; l <= LV; l++) bound[l] = (bound[l - 1] + B) / 2 + 1;
+    // the level-0 plan packs (table * stride + index) | sign << 31 into 32 bits (msm_affine.cuh aff_plan_thread)
+    B2M_REQUIRE(LV == 0 || (size_t)T * stride < ((size_t)1 << 31), B2M_ERR_DEGREE_TOO_LARGE,
+                "window tables of %d x %zu entries exceed the 31-bit index of the batched-affine plan", T, stride);
     DBuf<Affine<Fq>> lvl_pts[2];
     DBuf<uint32_t> lvl_off[2], lvl_cnt;
     DBuf<uint2> lvl_refs;
     DBuf<uint4> lvl_meta;
     DBuf<Fq> lvl_pref, lvl_inv;
     if (LV > 0) {
-      lvl_pts[0] = DBuf<Affine<Fq>>(cx, bound[1]);
-      if (LV > 1) lvl_pts[1] = DBuf<Affine<Fq>>(cx, bound[2]);
-      lvl_off[0] = DBuf<uint32_t>(cx, B + 1); lvl_off[1] = DBuf<uint32_t>(cx, B + 1); lvl_cnt = DBuf<uint32_t>(cx, B + 1);
+      lvl_pts[0] = DBuf<Affine<Fq>>(cx, lvl_cap[0]);
+      if (LV > 1) lvl_pts[1] = DBuf<Affine<Fq>>(cx, lvl_cap[1]);
+      lvl_off[0] = DBuf<uint32_t>(cx, NB + 1); lvl_off[1] = DBuf<uint32_t>(cx, NB + 1); lvl_cnt = DBuf<uint32_t>(cx, NB + 1);
       lvl_refs = DBuf<uint2>(cx, bound[LV]);
       const size_t T_max = (size_t)std::max(affine_T, affine_T_upper), T_min = (size_t)std::min(affine_T, affine_T_upper);
-      const size_t slots_l0 = T_max * ((bound[1] + T_max - 1) / T_max + 128);  // >= T * nthreads at every level, for either mapping
+      const size_t slots_l0 = T_max * ((std::max(lvl_cap[0], lvl_cap[1]) + T_max - 1) / T_max + 128);  // >= T * nthreads at every level, for either mapping
       lvl_meta = DBuf<uint4>(cx, slots_l0);
       lvl_pref = DBuf<Fq>(cx, slots_l0);
       lvl_inv = DBuf<Fq>(cx, slots_l0 / T_min + 256);
@@ -839,11 +942,11 @@ void Msm<Fr, Fq>::run_batch(const MsmJob<Fr, Fq>* jobs_in, int nj) {
         hist[s].zero();
         size_t sp0 = cx.span_begin("msm_sort", (double)n);
         msm_digits_kernel<Fr><<<div_up(nt, 256), 256, 0, cx.stream>>>(jobs[j].scalars, jobs[j].scalar_stride, jobs[j].scalars2, jobs[j].mont, n, nt, c, W,
-                                                                      digits[s].p, hist[s].p);
+                                                                      m, digits[s].p, hist[s].p);
         B2M_CHECK_LAUNCH();
-        exclusive_scan_u32(cx, hist[s].p, offsets[s].p, B + 1);  // hist[B] = 0: offsets[B] = number of references
-        B2M_CUDA(cudaMemcpyAsync(cursor[s].p, offsets[s].p, B * sizeof(uint32_t), cudaMemcpyDeviceToDevice, cx.stream));
-        msm_scatter_kernel<<<div_up(nt, 256), 256, 0, cx.stream>>>(digits[s].p, n, nt, jobs[j].base_off, n_srs + jobs[j].extra_base, W,
+        exclusive_scan_u32(cx, hist[s].p, offsets[s].p, NB + 1);  // hist[NB] = 0: offsets[NB] = number of references
+        B2M_CUDA(cudaMemcpyAsync(cursor[s].p, offsets[s].p, NB * sizeof(uint32_t), cudaMemcpyDeviceToDevice, cx.stream));
+        msm_scatter_kernel<<<div_up(nt, 256), 256, 0, cx.stream>>>(digits[s].p, n, nt, jobs[j].base_off, n_srs + jobs[j].extra_base, W, m,
                                                                     cursor[s].p, sorted[s].p);
         B2M_CHECK_LAUNCH();
         cx.launches += 2;
@@ -861,18 +964,18 @@ void Msm<Fr, Fq>::run_batch(const MsmJob<Fr, Fq>* jobs_in, int nj) {
       if (LV > 0 && refs >= affine_min_refs) {
         size_t spl = cx.span_begin("msm_affine_levels", (double)n);
         bound[0] = refs;
-        for (int l = 1; l <= LV; l++) bound[l] = (bound[l - 1] + B) / 2 + 1;
+        for (int l = 1; l <= LV; l++) bound[l] = (bound[l - 1] + NB) / 2 + 1;
         const uint32_t* off_in = offsets[s].p;
         for (int l = 0; l < LV; l++) {
           uint32_t* off_out = lvl_off[l & 1].p;
-          msm_level_counts_kernel<<<div_up((size_t)B + 1, 256), 256, 0, cx.stream>>>(off_in, B, lvl_cnt.p);
+          msm_level_counts_kernel<<<div_up((size_t)NB + 1, 256), 256, 0, cx.stream>>>(off_in, NB, lvl_cnt.p);
           B2M_CHECK_LAUNCH();
           cx.launches++;
-          exclusive_scan_u32(cx, lvl_cnt.p, off_out, (size_t)B + 1);
+          exclusive_scan_u32(cx, lvl_cnt.p, off_out, (size_t)NB + 1);
           const uint32_t lane_step = affine_map ? 32u : 1u;
           const size_t T_l = (size_t)(l == 0 ? affine_T : affine_T_upper);  // additions per thread (and per chain) at this level
           const uint32_t nthreads = (uint32_t)(lane_step * ((bound[l + 1] + (size_t)lane_step * T_l - 1) / ((size_t)lane_step * T_l)));
-          AffLevel<Fq> A{tables.p, stride, sorted[s].p, l > 0 ? lvl_pts[(l - 1) & 1].p : nullptr, off_in, off_out, B, lvl_pts[l & 1].p,
+          AffLevel<Fq> A{tables.p, stride, sorted[s].p, l > 0 ? lvl_pts[(l - 1) & 1].p : nullptr, off_in, off_out, NB, lvl_pts[l & 1].p,
                          l == LV - 1 ? lvl_refs.p : nullptr, lvl_pref.p, lvl_meta.p, (uint32_t)T_l, nthreads, lane_step, lvl_inv.p};
           if (l == 0)
             msm_affine_plan_kernel<Fq, true><<<div_up(nthreads, 256), 256, 0, cx.stream>>>(A);
@@ -924,7 +1027,7 @@ void Msm<Fr, Fq>::run_batch(const MsmJob<Fr, Fq>* jobs_in, int nj) {
         refs = bound[LV];
       }
       const uint32_t* src_ends = src_off + 1;   // buckets are contiguous: bucket b ends where b + 1 starts
-      const uint32_t* src_total = src_off + B;
+      const uint32_t* src_total = src_off + NB;
       size_t sp = cx.span_begin("msm_accumulate_kernel", (double)n);
       // References per thread: near MSM_Q, chosen so that the grid is a whole number of waves of
       // (SMs x resident CTAs) -- every thread does the same work, so a partial last wave is pure loss.
@@ -935,7 +1038,7 @@ void Msm<Fr, Fq>::run_batch(const MsmJob<Fr, Fq>* jobs_in, int nj) {
       if (q < (uint32_t)MSM_Q_MIN) q = MSM_Q_MIN;
       const size_t nthreads = (refs + q - 1) / q;
       msm_accumulate_kernel<Fq><<<div_up(nthreads, 128), 128, 0, cx.stream>>>(src_tables, src_stride, src_off, src_ends, src_sorted,
-                                                                               src_total, q, buckets.p + (size_t)j * B, part_pt.p,
+                                                                               src_total, q, buckets.p + (size_t)j * NB, part_pt.p,
                                                                                part_bkt.p);
       B2M_CHECK_LAUNCH();
       cx.launches++;
@@ -943,14 +1046,14 @@ void Msm<Fr, Fq>::run_batch(const MsmJob<Fr, Fq>* jobs_in, int nj) {
       size_t sp1 = cx.span_begin("msm_stitch", (double)n);
       n_long.zero();
       msm_stitch_kernel<Fq><<<div_up(nthreads, 128), 128, 0, cx.stream>>>(part_pt.p, part_bkt.p, nthreads, q, src_off, src_ends,
-                                                                           buckets.p + (size_t)j * B, long_runs.p, final_runs.p, short_runs.p, n_long.p,
+                                                                           buckets.p + (size_t)j * NB, long_runs.p, final_runs.p, short_runs.p, n_long.p,
                                                                            long_cap, chunk_cap);
       msm_stitch_short_kernel<Fq><<<2 * cx.sm_count, 128, 0, cx.stream>>>(part_pt.p, part_bkt.p, short_runs.p, n_long.p + 3, long_cap,
-                                                                          buckets.p + (size_t)j * B);
+                                                                          buckets.p + (size_t)j * NB);
       msm_stitch_runs_kernel<Fq, false><<<4 * cx.sm_count, 128, 0, cx.stream>>>(part_pt.p, part_bkt.p, long_runs.p, n_long.p, long_cap,
-                                                                                buckets.p + (size_t)j * B, chunk_pt.p);
+                                                                                buckets.p + (size_t)j * NB, chunk_pt.p);
       msm_stitch_runs_kernel<Fq, true><<<cx.sm_count, 128, 0, cx.stream>>>(part_pt.p, part_bkt.p, final_runs.p, n_long.p + 1, chunk_cap,
-                                                                           buckets.p + (size_t)j * B, chunk_pt.p);
+                                                                           buckets.p + (size_t)j * NB, chunk_pt.p);
       B2M_CHECK_LAUNCH();
       cx.launches += 4;
       cx.span_end(sp1);
@@ -965,26 +1068,34 @@ void Msm<Fr, Fq>::run_batch(const MsmJob<Fr, Fq>* jobs_in, int nj) {
   double units = 0;
   for (int j = 0; j < nj; j++) units += (double)jobs[j].n;
   size_t sp2 = cx.span_begin("msm_reduce", units);
-  DBuf<XYZZ<Fq>> rsum(cx, (size_t)nj * R), csum(cx, (size_t)nj * L);
+  DBuf<XYZZ<Fq>> rsum(cx, G * R), csum(cx, G * L);
   {
     // stage 1: K summands per thread (K = 8, or the whole axis when it is shorter); stage 2: one warp per position
     const uint32_t Kr = (uint32_t)std::min<size_t>(L, 8), Kc = (uint32_t)std::min<size_t>(R, 8);
     const size_t seg_r = L / Kr, seg_c = R / Kc;  // partials per row / per column
-    DBuf<XYZZ<Fq>> part_r(cx, (size_t)nj * R * seg_r), part_c(cx, (size_t)nj * L * seg_c);
-    msm_segsum_kernel<Fq><<<div_up((size_t)nj * R * seg_r, 128), 128, 0, cx.stream>>>(buckets.p, part_r.p, (size_t)nj, seg_r, Kr, R, 1, L, B);
-    msm_segsum_kernel<Fq><<<div_up((size_t)nj * L * seg_c, 128), 128, 0, cx.stream>>>(buckets.p, part_c.p, (size_t)nj, seg_c, Kc, L, L, 1, B);
-    const MsmFoldJob fr{part_r.p, rsum.p, (size_t)nj * R, seg_r}, fc{part_c.p, csum.p, (size_t)nj * L, seg_c};
-    msm_fold_kernel<Fq><<<div_up(((size_t)nj * R + (size_t)nj * L) * 32, 128), 128, 0, cx.stream>>>(fr, fc);
+    DBuf<XYZZ<Fq>> part_r(cx, G * R * seg_r), part_c(cx, G * L * seg_c);
+    msm_segsum_kernel<Fq><<<div_up(G * R * seg_r, 128), 128, 0, cx.stream>>>(buckets.p, part_r.p, G, seg_r, Kr, R, 1, L, B);
+    msm_segsum_kernel<Fq><<<div_up(G * L * seg_c, 128), 128, 0, cx.stream>>>(buckets.p, part_c.p, G, seg_c, Kc, L, L, 1, B);
+    const MsmFoldJob fr{part_r.p, rsum.p, G * R, seg_r}, fc{part_c.p, csum.p, G * L, seg_c};
+    msm_fold_kernel<Fq><<<div_up((G * R + G * L) * 32, 128), 128, 0, cx.stream>>>(fr, fc);
     B2M_CHECK_LAUNCH();
     cx.launches += 3;
   }
-  DBuf<XYZZ<Fq>> rplanes(cx, (size_t)nj * (rbits + 1)), cplanes(cx, (size_t)nj * (cbits + 1));
-  msm_bitplane_kernel<Fq><<<dim3(rbits + 1 + cbits + 1, nj), 256, 0, cx.stream>>>(rsum.p, R, rbits, rplanes.p, csum.p, L, cbits, cplanes.p);
+  DBuf<XYZZ<Fq>> rplanes(cx, G * (rbits + 1)), cplanes(cx, G * (cbits + 1));
+  msm_bitplane_kernel<Fq><<<dim3(rbits + 1 + cbits + 1, (unsigned)G), 256, 0, cx.stream>>>(rsum.p, R, rbits, rplanes.p, csum.p, L, cbits, cplanes.p);
   B2M_CHECK_LAUNCH();
   cx.launches++;
-  msm_finish_kernel<Fq><<<nj, 64, 0, cx.stream>>>(rplanes.p, rbits, cplanes.p, cbits, 1, fj);
-  B2M_CHECK_LAUNCH();
-  cx.launches++;
+  if (m == 1) {
+    msm_finish_kernel<Fq><<<nj, 64, 0, cx.stream>>>(rplanes.p, rbits, cplanes.p, cbits, 1, fj);
+    B2M_CHECK_LAUNCH();
+    cx.launches++;
+  } else {
+    DBuf<XYZZ<Fq>> set_sums(cx, G);
+    msm_set_sum_kernel<Fq><<<(unsigned)G, 64, 0, cx.stream>>>(rplanes.p, rbits, cplanes.p, cbits, set_sums.p);
+    msm_sets_finish_kernel<Fq><<<nj, 32, 0, cx.stream>>>(set_sums.p, m, c, fj);
+    B2M_CHECK_LAUNCH();
+    cx.launches += 2;
+  }
   cx.span_end(sp2);
   exchange();
   // the DBufs are stream-ordered: their frees are enqueued behind the kernels above

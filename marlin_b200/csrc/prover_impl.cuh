@@ -179,6 +179,7 @@ struct MarlinIndex : IndexBase {
     size_t md = std::max(std::max(2 * H - 1, 3 * H - 1), K - 1);  // reference src/ahp/mod.rs:83-92 with zk_bound = 1
     B2M_REQUIRE(D >= md, B2M_ERR_INDEX_TOO_LARGE, "SRS max degree %zu < index max degree %zu", D, md);
     B2M_REQUIRE(D >= K - 2 && D >= H - 2, B2M_ERR_INDEX_TOO_LARGE, "SRS too small for the degree bounds");
+    srs->require_fits(K, H);
     ntt.ensure_table(std::max(log_k + 1, log_h + 2));
     for (int i = 0; i < 6; i++) { ieval[i] = DBuf<Fr>(cx, K); ipoly[i] = DBuf<Fr>(cx, K); }
   }
