@@ -119,6 +119,7 @@ extern "C" {
     pub fn b2m_index_sizes(idx: *const b2m_index, num_non_zero: *mut usize, domain_k: *mut usize, matrix_nnz: *mut usize) -> c_int;
     pub fn b2m_index_export(idx: *mut b2m_index, vectors: *mut u8, row_ptrs: *const *mut u64, cols: *const *mut u64,
                             coeffs: *const *mut u8) -> c_int;
+    pub fn b2m_index_residency(idx: *const b2m_index, host: *mut c_int, host_bytes: *mut usize) -> c_int;
     pub fn b2m_fr_decode_ark(ctx: *mut b2m_ctx, curve: c_int, bytes: *const u8, n: usize, out_limbs: *mut u64, bad_index: *mut usize) -> c_int;
     pub fn b2m_fr_to_canonical(ctx: *mut b2m_ctx, curve: c_int, limbs: *const u64, n: usize, out: *mut u8) -> c_int;
     pub fn b2m_domain_ark(curve: c_int, log_size: c_uint, out: *mut u8) -> c_int;

@@ -345,6 +345,12 @@ int b2m_index_sizes(const b2m_index* idx, size_t* num_non_zero, size_t* domain_k
  * matrix m = A, B, C in the row form the index was given.  Any output pointer may be NULL to skip it. */
 int b2m_index_export(b2m_index* idx, uint8_t* vectors, uint64_t* const* row_ptrs, uint64_t* const* cols,
                      uint8_t* const* coeffs);
+/* Where the index keeps its twelve |K|-vectors: *host = 0 in device memory, 1 in pinned host memory, streamed to the GPU
+ * in round 3 and the opening of every proof; *host_bytes = the pinned bytes (0 when device-resident).  `index` and
+ * `load_index` choose host residency only when the device-memory model of the device-resident index does not fit and the
+ * host-resident one does (single-GPU contexts; environment B2M_INDEX_HOST=1 forces it, for tests).  Either pointer may be
+ * NULL. */
+int b2m_index_residency(const b2m_index* idx, int* host, size_t* host_bytes);
 
 
 /* Replaces `Marlin::prove` (reference src/lib.rs:151-311).  formatted_input: the instance

@@ -115,6 +115,7 @@ def lib():
             L.b2m_index_load.argtypes = [vp, ci, sz, sz, sz, sz, P(Matrix), P(Matrix), P(Matrix), vp, vp, vp, ci, P(sz), P(sz), P(ci), P(vp)]
             L.b2m_index_sizes.argtypes = [vp, P(sz), P(sz), vp]
             L.b2m_index_export.argtypes = [vp, vp, vp, vp, vp]
+            L.b2m_index_residency.argtypes = [vp, P(ci), P(sz)]
             L.b2m_index_stage.argtypes = [vp, vp, sz, vp, sz]
             L.b2m_prove.argtypes = [vp, vp, sz, vp, sz, P(Rng), vp, sz, P(sz)]
             L.b2m_prove_timings.argtypes = [vp, ctypes.c_char_p, sz]

@@ -230,6 +230,20 @@ class IndexProverKey:
         self.index_comms = np.zeros((6, 2 * lq), dtype=np.uint64)
         _lib.check(L.b2m_index_comms(handle, _lib.ptr(self.index_comms)))
 
+    @property
+    def residency(self):
+        """"device" or "host": where the index keeps its twelve |K|-vectors (b2m_index_residency)."""
+        host = ctypes.c_int(0)
+        _lib.check(_lib.lib().b2m_index_residency(self.handle, ctypes.byref(host), None))
+        return "host" if host.value else "device"
+
+    @property
+    def host_bytes(self):
+        """Pinned host bytes of a host-resident index (0 when device-resident)."""
+        n = ctypes.c_size_t(0)
+        _lib.check(_lib.lib().b2m_index_residency(self.handle, None, ctypes.byref(n)))
+        return n.value
+
     def timings(self):
         buf = ctypes.create_string_buffer(4096)
         _lib.check(_lib.lib().b2m_prove_timings(self.handle, buf, 4096))

@@ -669,6 +669,14 @@ int b2m_index_export(b2m_index* idx, uint8_t* vectors, uint64_t* const* row_ptrs
   });
 }
 
+int b2m_index_residency(const b2m_index* idx, int* host, size_t* host_bytes) {
+  return guard([&] {
+    B2M_REQUIRE(idx != nullptr, B2M_ERR_INVALID_ARG, "null argument");
+    if (host) *host = idx->impl->host_resident;
+    if (host_bytes) *host_bytes = idx->impl->host_bytes;
+  });
+}
+
 void b2m_index_destroy(b2m_index* idx) {
   if (!idx) return;
   b2m_srs* srs = idx->srs;

@@ -1,5 +1,6 @@
 // Definitions of the opaque handles of include/b2m.h and the host-buffer wrappers of Level 0.
 #pragma once
+#include <cstdio>
 #include <memory>
 #include <string>
 
@@ -85,7 +86,8 @@ struct b2m_srs {
   }
 
   // Layout of the key (msm_layout.hpp): all W window tables whenever the byte model of the largest circuit the key can index
-  // fits min(free device memory, the context's memory limit); else the largest T < W and MSM pass cap that fit; else
+  // fits min(free device memory, the context's memory limit); else the largest T < W and MSM pass cap that fit; only when no
+  // layout fits with a device-resident index, the same search with a host-resident one (layout.bytes.host_index); else
   // B2M_ERR_MEMORY_LIMIT before anything is allocated.  window_tables > 0 (or B2M_MSM_TABLES) forces T, B2M_MSM_MAX_PAIRS the
   // pass cap (tests).  A multi-GPU context keeps its tables sharded by rank instead: the full layout only.
   template <class Fr, class Fq>
@@ -118,7 +120,7 @@ struct b2m_srs {
                   forced_T, c_reduced, m, c_reduced - 1, MSM_BKT_BITS);
     }
     budget = cx.memory_budget();
-    layout = msm_plan_layout(shape, c_full, c_reduced, c_min, budget, forced_T, forced_cap);
+    layout = msm_plan_residency(shape, c_full, c_reduced, c_min, budget, forced_T, forced_cap);
     const MsmBytes& b = layout.bytes;
     B2M_REQUIRE(layout.T > 0, B2M_ERR_MEMORY_LIMIT,
                 "an SRS of %zu powers needs %zu bytes (window tables %zu, index and prover %zu, MSM scratch %zu at %d table(s), c = %d, "
@@ -126,18 +128,57 @@ struct b2m_srs {
                 n_g, b.total(), b.tables, b.circuit, b.msm, layout.T ? layout.T : 1, layout.c, layout.max_pairs, budget);
   }
 
-  // `index` of a circuit with |K| = K, |H| = H on this key: with a memory limit set, refuse before allocating when the model
-  // of its index, prover and MSM scratch (sized for this circuit's largest MSM, not the whole key) exceeds what the limit
-  // leaves.
-  void require_fits(size_t K, size_t H) const {
+  // Residency of an index of |K| = K, |H| = H on this key, before it allocates (true: the twelve |K|-vectors go to pinned host
+  // memory once the index is built).  Device residency whenever the model of its index, prover and MSM scratch (sized for this
+  // circuit's largest MSM, not the whole key) fits what the budget leaves; otherwise host residency if that model fits.  With
+  // a memory limit set and neither fitting, B2M_ERR_MEMORY_LIMIT naming both (without a limit the device-resident index is
+  // tried, as it always was).  force_host (B2M_INDEX_HOST, tests) takes host residency whatever fits.  Host residency is
+  // refused when MemAvailable (/proc/meminfo) is below the bytes it pins, and on multi-GPU contexts.  held: bytes the index
+  // already took for structures the model's index term counts (its matrices), added back to the budget.
+  bool require_fits(size_t K, size_t H, bool force_host, size_t held) const {
     using namespace b2m;
     Ctx& cx = ctx->cx;
-    if (!cx.memory_limit || cx.world > 1) return;
-    const MsmBytes b = msm_model_bytes(shape, layout.c, layout.T, layout.max_pairs, K, H);
-    const size_t avail = cx.memory_budget();
-    B2M_REQUIRE(b.circuit + b.msm <= avail, B2M_ERR_MEMORY_LIMIT,
-                "an index of |K| = %zu, |H| = %zu needs %zu bytes (index and prover %zu, MSM scratch %zu); the device-memory budget leaves %zu bytes",
-                K, H, b.circuit + b.msm, b.circuit, b.msm, avail);
+    if (cx.world > 1) {
+      B2M_REQUIRE(!force_host, B2M_ERR_UNSUPPORTED, "a host-resident index needs a single-GPU context (this one is rank %d of %d)", cx.rank, cx.world);
+      return false;
+    }
+    const MsmBytes d = msm_model_bytes(shape, layout.c, layout.T, layout.max_pairs, K, H, false);
+    const MsmBytes h = msm_model_bytes(shape, layout.c, layout.T, layout.max_pairs, K, H, true);
+    bool host = force_host;
+    const size_t avail = cx.memory_budget() + held;
+    if (!host && d.circuit + d.msm > avail) {
+      host = h.circuit + h.msm <= avail;
+      B2M_REQUIRE(host || !cx.memory_limit, B2M_ERR_MEMORY_LIMIT,
+                  "an index of |K| = %zu, |H| = %zu needs %zu bytes device-resident (index and prover %zu, MSM scratch %zu) or %zu bytes "
+                  "host-resident (index and prover %zu, %zu bytes pinned on the host); the device-memory budget leaves %zu bytes",
+                  K, H, d.circuit + d.msm, d.circuit, d.msm, h.circuit + h.msm, h.circuit, h.host, avail);
+    }
+    if (host && cx.memory_limit)
+      B2M_REQUIRE(h.circuit + h.msm <= avail, B2M_ERR_MEMORY_LIMIT,
+                  "a host-resident index of |K| = %zu, |H| = %zu needs %zu bytes (index and prover %zu, MSM scratch %zu); the device-memory "
+                  "budget leaves %zu bytes", K, H, h.circuit + h.msm, h.circuit, h.msm, avail);
+    if (host) {
+      const size_t mem = host_mem_available();
+      B2M_REQUIRE(h.host <= mem, B2M_ERR_MEMORY_LIMIT, "a host-resident index of |K| = %zu pins %zu bytes of host memory; MemAvailable is %zu bytes", K,
+                  h.host, mem);
+    }
+    return host;
+  }
+  // MemAvailable of /proc/meminfo in bytes (SIZE_MAX when it cannot be read)
+  static size_t host_mem_available() {
+    FILE* f = fopen("/proc/meminfo", "r");
+    if (!f) return (size_t)-1;
+    char line[256];
+    size_t kb = (size_t)-1;
+    while (fgets(line, sizeof line, f)) {
+      unsigned long long v = 0;
+      if (sscanf(line, "MemAvailable: %llu kB", &v) == 1) {
+        kb = (size_t)v;
+        break;
+      }
+    }
+    fclose(f);
+    return kb == (size_t)-1 ? kb : kb * 1024;
   }
   int window_bits() const { return bls ? bls->c : bn->c; }
   int window_tables() const { return bls ? bls->T : bn->T; }

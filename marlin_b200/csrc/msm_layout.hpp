@@ -48,8 +48,15 @@ struct MsmBytes {
   size_t tables = 0;   // the T window tables
   size_t circuit = 0;  // index structures plus the larger of the index-build temporaries and the prover's buffers
   size_t msm = 0;      // scratch of one run_batch call of MSM_MAX_BATCH jobs, each pass as large as the cap allows
+  bool host_index = false;  // the circuit term keeps the twelve |K|-vectors of the index in pinned host memory
+  size_t host = 0;          // pinned host bytes of a host-resident index (not part of total())
   size_t total() const { return tables + circuit + msm + MSM_POOL_SLACK; }
 };
+
+// A host-resident index streams its vectors to the prover in chunks of this many Fr, two device slots per streamed vector
+// (round 3 streams at most three vectors at once).
+constexpr size_t INDEX_STREAM_CHUNK = (size_t)1 << 20;
+constexpr int INDEX_STREAM_VECS = 3;
 
 // Largest circuit a key of n_g powers can index: |K| - 1 <= D and 3 |H| - 1 <= D (D = n_g - 1, AHP max degree, zk bound 1).
 inline size_t msm_pow2_floor(size_t x) {
@@ -66,22 +73,42 @@ inline size_t msm_largest_pairs(size_t n_g, size_t K, size_t H) { return std::mi
 
 // THE byte model: an upper bound on the stream-ordered pool bytes that a key of layout (c, T, max_pairs) holds together with
 // the index and one proof of a circuit with |K| = K, |H| = H, at the peak of `index` or `prove`.  Written from the allocation
-// sites; every term names them.
-inline MsmBytes msm_model_bytes(const MsmKeyShape& k, int c, int T, size_t max_pairs, size_t K, size_t H) {
+// sites; every term names them.  host_index: the index keeps its twelve |K|-vectors in pinned host memory once it is built.
+inline MsmBytes msm_model_bytes(const MsmKeyShape& k, int c, int T, size_t max_pairs, size_t K, size_t H, bool host_index = false) {
   const size_t fr = 32, aff = 2 * k.fq_bytes, xyzz = 4 * k.fq_bytes;
   const int W = msm_windows(k.fr_bits, c), m = msm_sets(W, T);
   T = msm_tables_used(W, T);
   MsmBytes b;
   b.tables = (size_t)T * (k.n_g + k.n_extra) * aff;  // Msm::tables
-  // prover_impl.cuh.  Resident index: ieval / ipoly (12 K Fr), the CSR of A and B (each matrix has at most K entries), the
-  // column buckets of A, B, C for t(X), the NTT twiddles (half of the largest domain, max(2K, 4H)).
-  const size_t index = 12 * K * fr + 2 * (4 * (H + 1) + K * (4 + fr)) + 4 * (H + 1) + 3 * K * (4 + 1 + fr) + std::max(K, 2 * H) * fr;
-  // Index build (5 nnz vectors of the joint matrix, the work and evaluation vectors) versus one proof: rounds 1-2 hold about
-  // 40 vectors of |H| (z, z_A, z_B, masks, the 4|H| evaluation vectors of the first and second sumchecks), round 3 about 11
-  // of |K| (f, h_2 and their 2|K| evaluations) plus t(X)'s 3|K| products; the sum of both bounds either peak.
+  // prover_impl.cuh.  Resident index: ieval / ipoly (12 K Fr, `vecs`), the CSR of A and B (each matrix has at most K entries),
+  // the column buckets of A, B, C for t(X), the NTT twiddles (half of the largest domain, max(2K, 4H)).
+  const size_t vecs = 12 * K * fr;
+  const size_t index = 2 * (4 * (H + 1) + K * (4 + fr)) + 4 * (H + 1) + 3 * K * (4 + 1 + fr) + std::max(K, 2 * H) * fr;
+  // Index build (5 nnz vectors of the joint matrix, the work and evaluation vectors; load: the evaluation and NTT work
+  // vectors), always with the twelve vectors on the device.
   const size_t build = 3 * K * (8 + 3 * fr) + 2 * K * fr;
-  const size_t prove = (48 * H + 20 * K) * fr;
-  b.circuit = index + std::max(build, prove);
+  // One proof, the largest of its phases (in units of Fr; every vector of |H| or |H| + 1 counted as H + 1):
+  //  * alive from rounds 1-2 to the end: the staged and the proof's z, z_A, z_B, x(X), w(X), z_A(X), z_B(X), the 3|H| mask,
+  //    the 4|H| `summed` evaluations, r(alpha, X) evaluations and coefficients, t(X), z(X), g_1, the 2|H| h_1: 22 (H + 1);
+  //  * rounds 1-2: the four 4|H| vectors of q_1 and fft_padded's 4|H| work vector: 20 (H + 1) more (round 1's mask sampling,
+  //    t(X)'s 3|K| products and the 4|H| evaluations of z_A, z_B are freed before them and smaller: 5H, 3K + H and 12H);
+  //  * round 3: f, h_2; b, f evaluations and b(X); the three 2|K| vectors of b f and fft_padded's 2|K| work vector: 13 K;
+  //  * the opening: the evaluations' suffix vectors of g_1, g_2 and z_b / t (2 (H + 1) + K), and per point the combination,
+  //    its suffix sums and at most the merged witness scalars (4 n; n = 3|H| at beta, |K| at gamma), besides f and h_2.
+  const size_t live = 22 * (H + 1);
+  const size_t r12 = live + 20 * (H + 1);
+  const size_t r3 = live + 13 * K;
+  const size_t open = live + 2 * (H + 1) + 3 * K + 12 * (H + 1) + 4 * K;
+  const size_t prove = std::max(std::max(r12, r3), open) * fr;
+  // A host-resident index at rest holds no |K|-vector; round 3 and the opening stream them through the stager's slots.
+  const size_t stager = 2 * (size_t)INDEX_STREAM_VECS * std::min(K, INDEX_STREAM_CHUNK) * fr;
+  if (host_index) {
+    b.circuit = std::max(index + vecs + build, index + prove + stager);
+    b.host_index = true;
+    b.host = vecs;
+  } else {
+    b.circuit = index + vecs + std::max(build, prove);
+  }
   // msm_impl.cuh run_batch: the circuit's largest MSM (plus a few blinding pairs), or one pass of max_pairs pairs.
   const size_t nb = (size_t)m << (c - 1);  // buckets per MSM
   const size_t largest = msm_largest_pairs(k.n_g, K, H);
@@ -105,8 +132,8 @@ inline MsmBytes msm_model_bytes(const MsmKeyShape& k, int c, int T, size_t max_p
   b.msm = s;
   return b;
 }
-inline MsmBytes msm_model_bytes_largest(const MsmKeyShape& k, int c, int T, size_t max_pairs) {
-  return msm_model_bytes(k, c, T, max_pairs, msm_largest_k(k.n_g), msm_largest_h(k.n_g));
+inline MsmBytes msm_model_bytes_largest(const MsmKeyShape& k, int c, int T, size_t max_pairs, bool host_index = false) {
+  return msm_model_bytes(k, c, T, max_pairs, msm_largest_k(k.n_g), msm_largest_h(k.n_g), host_index);
 }
 
 struct MsmLayout {
@@ -120,8 +147,10 @@ struct MsmLayout {
 // below the full W at the widest window in [c_min, c_reduced] that fits, again with the largest cap that fits.  Only
 // T = ceil(W / m) are considered (msm_tables_used): any other T has the sets of the next such T and idle tables.  forced_T /
 // forced_cap (> 0) fix those choices (forced_T >= W: the full layout; other T normalised); c_min = c_reduced = c_full fixes
-// the window.  When nothing fits, T = 0 and `bytes` holds the smallest layout's figures.
-inline MsmLayout msm_plan_layout(const MsmKeyShape& k, int c_full, int c_reduced, int c_min, size_t budget, int forced_T, size_t forced_cap) {
+// the window.  When nothing fits, T = 0 and `bytes` holds the smallest layout's figures.  host_index: the circuit term of a
+// host-resident index (msm_model_bytes).
+inline MsmLayout msm_plan_layout(const MsmKeyShape& k, int c_full, int c_reduced, int c_min, size_t budget, int forced_T, size_t forced_cap,
+                                 bool host_index = false) {
   MsmLayout best;
   auto caps_try = [&](int c, int T, MsmLayout& out) {
     for (int lg = MSM_PASS_LOG_MAX + 1; lg >= MSM_PASS_LOG_MIN; lg--) {
@@ -132,7 +161,7 @@ inline MsmLayout msm_plan_layout(const MsmKeyShape& k, int c_full, int c_reduced
       } else if (cap && cap >= k.n_g) {
         continue;  // no cap
       }
-      const MsmBytes b = msm_model_bytes_largest(k, c, T, cap);
+      const MsmBytes b = msm_model_bytes_largest(k, c, T, cap, host_index);
       out = MsmLayout{c, msm_windows(k.fr_bits, c), T, cap, b};
       if (b.total() <= budget) return true;
     }
@@ -161,6 +190,18 @@ inline MsmLayout msm_plan_layout(const MsmKeyShape& k, int c_full, int c_reduced
   }
   best.T = 0;
   return best;
+}
+
+// Residency rule: exactly the device-resident search first (every T and pass cap); only when nothing fits, the same search
+// with the index's twelve |K|-vectors in pinned host memory.  The result's bytes.host_index records which one planned it;
+// when neither fits, T = 0 and `bytes` holds the device search's smallest layout.  (So the tables kept are monotone in the
+// budget within each residency, not across the switch: a host-resident plan may keep more tables than the device-resident
+// plan of a slightly larger budget.)
+inline MsmLayout msm_plan_residency(const MsmKeyShape& k, int c_full, int c_reduced, int c_min, size_t budget, int forced_T, size_t forced_cap) {
+  const MsmLayout dev = msm_plan_layout(k, c_full, c_reduced, c_min, budget, forced_T, forced_cap, false);
+  if (dev.T > 0) return dev;
+  const MsmLayout host = msm_plan_layout(k, c_full, c_reduced, c_min, budget, forced_T, forced_cap, true);
+  return host.T > 0 ? host : dev;
 }
 
 }  // namespace b2m

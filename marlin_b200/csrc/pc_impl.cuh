@@ -145,16 +145,118 @@ struct WitnessMsms {
 };
 
 // A labelled polynomial living in HBM, with its commitment and its kzg10::Randomness (host blinding polynomials; empty when
-// it is not hiding).
+// it is not hiding).  A host-resident index's polynomials live in pinned host memory instead (`host`): pc_open streams them.
 template <class Fr, class Fq>
 struct LabeledPoly {
   const Fr* p = nullptr;
   size_t len = 0;
+  bool host = false;    // p is pinned host memory (an index polynomial of a host-resident index; never bounded or hiding)
   int64_t bound = -1;   // degree bound, or -1
   int64_t hiding = -1;  // hiding bound, or -1
   std::vector<Fr> rand, shifted_rand;
   Affine<Fq> comm, shifted_comm;  // shifted_comm: MarlinKZG10, bounded polynomials only (the identity otherwise)
 };
+
+// Streams vectors held in pinned host memory to the device in chunks of INDEX_STREAM_CHUNK elements, double-buffered: chunk
+// j of every vector is copied into slot j % 2 on the index's own copy stream (not cx.side, which the MSM's counting sort
+// uses) while the consumer of chunk j - 1 reads the other slot on cx.stream.  Events order each slot's copy before its
+// consumer and the consumer before the slot's next copy.  Each vector crosses PCIe once per call.
+template <class Fr>
+struct HostStager {
+  Ctx& cx;
+  cudaStream_t copy;
+  size_t bytes = 0;                                          // streamed by this stager
+  std::vector<std::pair<cudaEvent_t, cudaEvent_t>> copies;   // first to last copy of each call, on the copy stream
+  HostStager(Ctx& c, cudaStream_t s) : cx(c), copy(s) {}
+  HostStager(const HostStager&) = delete;
+  ~HostStager() {
+    for (auto& e : copies) {
+      cudaEventDestroy(e.first);
+      cudaEventDestroy(e.second);
+    }
+  }
+  // milliseconds the copy engine spent on the calls so far (waits for them)
+  double copy_ms() {
+    double ms = 0;
+    for (auto& e : copies) {
+      float t = 0;
+      B2M_CUDA(cudaEventSynchronize(e.second));
+      B2M_CUDA(cudaEventElapsedTime(&t, e.first, e.second));
+      ms += t;
+    }
+    return ms;
+  }
+  // consume(slot, stride, at, m) launches on cx.stream a kernel reading elements [at, at + m) of vector v at slot + v * stride
+  template <class F>
+  void stream(const char* span, const Fr* const* src, int nv, size_t n, F&& consume) {
+    if (n == 0 || nv == 0) return;
+    B2M_REQUIRE(nv <= INDEX_STREAM_VECS, B2M_ERR_INVALID_ARG, "%d streamed vectors, at most %d", nv, INDEX_STREAM_VECS);
+    const size_t chunk = std::min(n, INDEX_STREAM_CHUNK);
+    DBuf<Fr> slot[2] = {DBuf<Fr>(cx, nv * chunk), DBuf<Fr>(cx, nv * chunk)};
+    cudaEvent_t ready, copied[2], consumed[2], t0, t1;
+    B2M_CUDA(cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
+    for (int s = 0; s < 2; s++) {
+      B2M_CUDA(cudaEventCreateWithFlags(&copied[s], cudaEventDisableTiming));
+      B2M_CUDA(cudaEventCreateWithFlags(&consumed[s], cudaEventDisableTiming));
+    }
+    B2M_CUDA(cudaEventCreate(&t0));
+    B2M_CUDA(cudaEventCreate(&t1));
+    B2M_CUDA(cudaEventRecord(ready, cx.stream));  // the slots' stream-ordered allocation, and whatever came before
+    B2M_CUDA(cudaStreamWaitEvent(copy, ready, 0));
+    B2M_CUDA(cudaEventRecord(t0, copy));
+    Ctx::Span prof{"index_h2d", 0.0, nullptr, nullptr};  // b2m_ctx_profile: the copies as a span of their own, on the copy stream
+    if (cx.profiling) {
+      B2M_CUDA(cudaEventCreate(&prof.a));
+      B2M_CUDA(cudaEventCreate(&prof.b));
+      B2M_CUDA(cudaEventRecord(prof.a, copy));
+    }
+    for (size_t at = 0, j = 0; at < n; at += chunk, j++) {
+      const int s = (int)(j & 1);
+      const size_t m = std::min(chunk, n - at);
+      if (j >= 2) B2M_CUDA(cudaStreamWaitEvent(copy, consumed[s], 0));
+      for (int v = 0; v < nv; v++)
+        B2M_CUDA(cudaMemcpyAsync(slot[s].p + v * chunk, src[v] + at, m * sizeof(Fr), cudaMemcpyHostToDevice, copy));
+      if (at + m == n) {  // the last copy: timed before the event cx.stream waits on, so a sync of cx.stream covers them
+        B2M_CUDA(cudaEventRecord(t1, copy));
+        if (cx.profiling) B2M_CUDA(cudaEventRecord(prof.b, copy));
+      }
+      B2M_CUDA(cudaEventRecord(copied[s], copy));
+      B2M_CUDA(cudaStreamWaitEvent(cx.stream, copied[s], 0));
+      const size_t sp = cx.span_begin(span, (double)m);
+      consume((const Fr*)slot[s].p, chunk, at, m);
+      cx.span_end(sp);
+      B2M_CUDA(cudaEventRecord(consumed[s], cx.stream));
+    }
+    const size_t moved = (size_t)nv * n * sizeof(Fr);
+    bytes += moved;
+    copies.push_back({t0, t1});
+    if (cx.profiling) {
+      prof.units = (double)moved;
+      cx.spans.push_back(prof);
+    }
+    // (destroying an event still pending in a stream releases it once it completes)
+    cudaEventDestroy(ready);
+    for (int s = 0; s < 2; s++) {
+      cudaEventDestroy(copied[s]);
+      cudaEventDestroy(consumed[s]);
+    }
+  }
+};
+
+// out[at + i] += sum_t c[t] * slot[t * stride + i], i < m: host terms of a combination, one streamed chunk at a time
+template <class Fr>
+struct StreamTerms {
+  Fr c[INDEX_STREAM_VECS];
+  int n;
+};
+template <class Fr>
+__global__ void index_stream_lincomb_kernel(StreamTerms<Fr> t, const Fr* __restrict__ slot, size_t stride, size_t m, Fr* out) {
+  const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= m) return;
+  Fr acc = ld_fr(out + i);
+  for (int k = 0; k < t.n; k++) acc = acc + t.c[k] * ld_fr(slot + k * stride + i);
+  st_fr(out + i, acc);
+}
 
 // `PC::commit`: draws the blinding polynomials from zk in the reference's order (per polynomial: its randomness, then, for a
 // bounded polynomial under MarlinKZG10, its shifted randomness) and runs the KZG10 commitments in batches of MSM_MAX_BATCH.
@@ -234,9 +336,12 @@ struct Opening {
 // `PC::open_combinations` [U marlin_pc / sonic_pc open_combinations_individual_opening_challenges] at every point at once.  At
 // each point the opening challenges xi^0, xi^1, .. go to its combinations in order, and under MarlinKZG10 one more to the
 // shifted part of each bounded one.  A point's combination sum_k ch_k * lc_k is formed by as few lincomb_kernel launches as
-// hold its terms; the witness MSMs of all points share one WitnessMsms and all witnesses come back in one download.
+// hold its terms; the witness MSMs of all points share one WitnessMsms and all witnesses come back in one download.  Terms in
+// pinned host memory (LabeledPoly::host, which needs a stager) are added to the combination afterwards, streamed chunk by
+// chunk, INDEX_STREAM_VECS at a time.
 template <class Fr, class Fq>
-std::vector<Opening<Fr, Fq>> pc_open(b2m_srs* srs, Msm<Fr, Fq>& msm, int pc, const Fr& xi, const std::vector<OpenPoint<Fr, Fq>>& points) {
+std::vector<Opening<Fr, Fq>> pc_open(b2m_srs* srs, Msm<Fr, Fq>& msm, int pc, const Fr& xi, const std::vector<OpenPoint<Fr, Fq>>& points,
+                                     HostStager<Fr>* stager = nullptr) {
   typedef typename WitnessMsms<Fr, Fq>::Shifted Shifted;
   Ctx& cx = srs->ctx->cx;
   const size_t D = srs->n_g - 1;
@@ -252,7 +357,7 @@ std::vector<Opening<Fr, Fq>> pc_open(b2m_srs* srs, Msm<Fr, Fq>& msm, int pc, con
       size_t len;
       Fr c;
     };
-    std::vector<Weighted> flat;
+    std::vector<Weighted> flat, host;
     std::vector<Shifted> shifted;
     std::vector<Fr> r, sr, srw;  // combined randomness, shifted randomness, shifted randomness / (X - z)
     size_t n = 1;
@@ -260,7 +365,7 @@ std::vector<Opening<Fr, Fq>> pc_open(b2m_srs* srs, Msm<Fr, Fq>& msm, int pc, con
     for (const auto& lc : points[p].lcs) {
       std::vector<Fr> lr;
       for (const auto& t : lc.terms) {
-        flat.push_back(Weighted{t.poly->p, t.poly->len, ch * t.coef});
+        (t.poly->host ? host : flat).push_back(Weighted{t.poly->p, t.poly->len, ch * t.coef});
         n = std::max(n, t.poly->len);
         hp_axpy(lr, t.coef, t.poly->rand);
       }
@@ -288,6 +393,28 @@ std::vector<Opening<Fr, Fq>> pc_open(b2m_srs* srs, Msm<Fr, Fq>& msm, int pc, con
       if (at > 0) lt.add(comb.p, n, one);
       for (; lt.n < LcTerms<Fr>::MAX && at < flat.size(); at++) lt.add(flat[at].src, flat[at].len, flat[at].c);
       launch_lincomb(cx, lt, n, comb.p);
+    }
+    if (!host.empty()) {
+      B2M_REQUIRE(stager != nullptr, B2M_ERR_INVALID_ARG, "a host-resident polynomial needs a stager");
+      for (size_t at = 0; at < host.size(); at += INDEX_STREAM_VECS) {
+        const Fr* src[INDEX_STREAM_VECS];
+        StreamTerms<Fr> st;
+        st.n = (int)std::min<size_t>(INDEX_STREAM_VECS, host.size() - at);
+        size_t len = 0;
+        for (int k = 0; k < st.n; k++) {
+          src[k] = host[at + k].src;
+          st.c[k] = host[at + k].c;
+          len = std::max(len, host[at + k].len);
+        }
+        for (int k = 0; k < st.n; k++)
+          B2M_REQUIRE(host[at + k].len == len, B2M_ERR_INVALID_ARG, "streamed terms of one pass differ in length");
+        Fr* out = comb.p;
+        stager->stream("index_open_lincomb", src, st.n, len, [&](const Fr* slot, size_t stride, size_t off, size_t m) {
+          index_stream_lincomb_kernel<Fr><<<div_up(m, 256), 256, 0, cx.stream>>>(st, slot, stride, m, out + off);
+          B2M_CHECK_LAUNCH();
+          cx.launches++;
+        });
+      }
     }
     // S[0] = comb(z), S[1 ..] = comb / (X - z): the plain witness; r / (X - z) plus the shifted part: the hiding witness
     rec_suffix<Fr>(cx, comb.p, sfx.p, n, 1, z, true);

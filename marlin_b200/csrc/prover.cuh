@@ -20,6 +20,8 @@ struct IndexBase {
   virtual void sizes(size_t* num_non_zero, size_t* domain_k, size_t* matrix_nnz) const = 0;
   // b2m_index_export
   virtual void export_keys(uint8_t* vectors, uint64_t* const* row_ptrs, uint64_t* const* cols, uint8_t* const* coeffs) = 0;
+  int host_resident = 0;            // the twelve |K|-vectors live in pinned host memory (b2m_index_residency)
+  size_t host_bytes = 0;            // their pinned bytes
   std::vector<uint8_t> vk_bytes;    // IndexVerifierKey::write (ToBytes)
   std::vector<uint64_t> comms_xy;   // six index commitments, affine Montgomery limbs
   std::string timings_json;

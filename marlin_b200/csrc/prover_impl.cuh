@@ -27,6 +27,25 @@
 
 namespace b2m {
 
+// Round 3 of a host-resident index, over one streamed chunk: b|_K = f|_K = (beta - row)(alpha - col) before the batch
+// inversion, and f|_K *= eta_a v a_val + eta_b v b_val + eta_c v c_val after it (the device-resident index runs the same
+// arithmetic as two whole-vector elementwise kernels).
+template <class Fr>
+__global__ void index_r3_denominators_kernel(const Fr* __restrict__ row, const Fr* __restrict__ col, size_t m, Fr alpha, Fr beta, Fr* b_ev,
+                                             Fr* f_ev) {
+  const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= m) return;
+  const Fr d = (beta - ld_fr(row + i)) * (alpha - ld_fr(col + i));
+  st_fr(b_ev + i, d);
+  st_fr(f_ev + i, d);
+}
+template <class Fr>
+__global__ void index_r3_f_kernel(const Fr* __restrict__ slot, size_t stride, size_t m, Fr ea, Fr eb, Fr ec, Fr* f_ev) {
+  const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= m) return;
+  st_fr(f_ev + i, ld_fr(f_ev + i) * (ea * ld_fr(slot + i) + eb * ld_fr(slot + stride + i) + ec * ld_fr(slot + 2 * stride + i)));
+}
+
 template <class Fr, class Fq>
 struct MarlinIndex : IndexBase {
   using Pt = Affine<Fq>;
@@ -51,6 +70,19 @@ struct MarlinIndex : IndexBase {
   size_t t_entries = 0;
   DBuf<Fr> ipoly[6], ieval[6];  // row, col, a_val, b_val, c_val, row_col (coefficients / evaluations on K)
   LP index_polys[6];  // ipoly with their commitments
+  // A host-resident index (require_fits, B2M_INDEX_HOST) moves the twelve vectors above into one pinned allocation once it is
+  // built or loaded: ipoly[i] at hvec + i K, ieval[i] at hvec + (6 + i) K.  Round 3 and the opening stream them on copy_stream.
+  Fr* hvec = nullptr;
+  cudaStream_t copy_stream = nullptr;
+  bool force_host = false;
+  const Fr* vec(int v) const { return hvec ? hvec + (size_t)v * K : (v < 6 ? ipoly[v].p : ieval[v - 6].p); }
+  ~MarlinIndex() override {
+    if (copy_stream) {
+      cudaStreamSynchronize(copy_stream);
+      cudaStreamDestroy(copy_stream);
+    }
+    if (hvec) cudaFreeHost(hvec);
+  }
 
   struct Timer {
     Ctx& cx;
@@ -101,7 +133,9 @@ struct MarlinIndex : IndexBase {
   // `Marlin::index`: AHPForR1CS::index + trim + commit
   // ---------------------------------------------------------------------------------------------
   MarlinIndex(b2m_srs* s, Ntt<Fr>& ntt_, Msm<Fr, Fq>& msm_, int pc_, size_t nc_, size_t nv_, size_t ni_)
-      : srs(s), cx(s->ctx->cx), ntt(ntt_), msm(msm_), pc(pc_), nc(nc_), nv(nv_), ni(ni_) {}
+      : srs(s), cx(s->ctx->cx), ntt(ntt_), msm(msm_), pc(pc_), nc(nc_), nv(nv_), ni(ni_) {
+    if (const char* e = getenv("B2M_INDEX_HOST")) force_host = atoi(e) != 0;  // tests: host residency whatever fits
+  }
 
   // The matrices as the index received them (row form, Montgomery coefficients): kept for export (b2m_index_export).
   std::vector<uint64_t> m_rowptr[3], m_col[3], m_coeff[3];
@@ -179,7 +213,10 @@ struct MarlinIndex : IndexBase {
     size_t md = std::max(std::max(2 * H - 1, 3 * H - 1), K - 1);  // reference src/ahp/mod.rs:83-92 with zk_bound = 1
     B2M_REQUIRE(D >= md, B2M_ERR_INDEX_TOO_LARGE, "SRS max degree %zu < index max degree %zu", D, md);
     B2M_REQUIRE(D >= K - 2 && D >= H - 2, B2M_ERR_INDEX_TOO_LARGE, "SRS too small for the degree bounds");
-    srs->require_fits(K, H);
+    // (prepare()'s buffers are in the model's index term already: they count as room, not as pool bytes in use)
+    const size_t held = (a_rowptr.n + a_col.n + b_rowptr.n + b_col.n + t_colptr.n + t_row.n) * 4 + t_mat.n +
+                        (a_coeff.n + b_coeff.n + t_coeff.n) * sizeof(Fr);
+    host_resident = srs->require_fits(K, H, force_host, held) ? 1 : 0;
     ntt.ensure_table(std::max(log_k + 1, log_h + 2));
     for (int i = 0; i < 6; i++) { ieval[i] = DBuf<Fr>(cx, K); ipoly[i] = DBuf<Fr>(cx, K); }
   }
@@ -192,6 +229,24 @@ struct MarlinIndex : IndexBase {
     vk_bytes.clear();
     put_u64(vk_bytes, nv); put_u64(vk_bytes, nc); put_u64(vk_bytes, nnz);
     for (int i = 0; i < 6; i++) write_commitment(vk_bytes, index_polys[i].comm, false, Pt::inf());
+  }
+  // The end of build() and load() for a host-resident index, after the commitments and the key-file checks: the twelve
+  // vectors go to one pinned allocation and their device buffers back to the pool.
+  void move_to_host() {
+    if (!host_resident) return;
+    const size_t bytes = 12 * K * sizeof(Fr);
+    B2M_CUDA(cudaHostAlloc((void**)&hvec, bytes, cudaHostAllocDefault));
+    host_bytes = bytes;
+    for (int v = 0; v < 12; v++)
+      B2M_CUDA(cudaMemcpyAsync(hvec + (size_t)v * K, v < 6 ? ipoly[v].p : ieval[v - 6].p, K * sizeof(Fr), cudaMemcpyDeviceToHost, cx.stream));
+    cx.sync();
+    for (int i = 0; i < 6; i++) {
+      ipoly[i].release();
+      ieval[i].release();
+      index_polys[i].p = hvec + (size_t)i * K;
+      index_polys[i].host = true;
+    }
+    B2M_CUDA(cudaStreamCreateWithFlags(&copy_stream, cudaStreamNonBlocking));
   }
   void bind_index_polys() {
     for (int i = 0; i < 6; i++) {
@@ -272,6 +327,7 @@ struct MarlinIndex : IndexBase {
     ZkSource<b2m_rng> no_rng(nullptr);
     pc_commit(srs, msm, pc, ips, no_rng);
     finish_vk();
+    move_to_host();
   }
 
   // An index from a key file (b2m_index_load): the matrices give the same derived structures as build(); the twelve index
@@ -347,6 +403,7 @@ struct MarlinIndex : IndexBase {
         }
     }
     finish_vk();
+    move_to_host();
   }
 
   void sizes(size_t* out_nnz, size_t* out_k, size_t* matrix_nnz) const override {
@@ -357,8 +414,18 @@ struct MarlinIndex : IndexBase {
   // b2m_index_export: the twelve vectors (K canonical Fr each, coefficients zero-padded) and the matrices in row form with
   // canonical coefficients, both converted on the device
   void export_keys(uint8_t* vectors, uint64_t* const* row_ptrs, uint64_t* const* cols, uint8_t* const* coeffs) override {
-    if (vectors)
+    if (vectors && !hvec)
       for (int v = 0; v < 12; v++) fr_to_canonical<Fr>(cx, v < 6 ? ipoly[v].p : ieval[v - 6].p, K, vectors + (size_t)v * K * sizeof(Fr));
+    if (vectors && hvec) {  // host-resident: through one device chunk
+      const size_t chunk = std::min(K, INDEX_STREAM_CHUNK);
+      DBuf<Fr> d(cx, chunk);
+      for (int v = 0; v < 12; v++)
+        for (size_t at = 0; at < K; at += chunk) {
+          const size_t m = std::min(chunk, K - at);
+          d.upload(vec(v) + at, m);
+          fr_to_canonical<Fr>(cx, d.p, m, vectors + ((size_t)v * K + at) * sizeof(Fr));
+        }
+    }
     for (int m = 0; m < 3; m++) {
       if (row_ptrs && row_ptrs[m]) memcpy(row_ptrs[m], m_rowptr[m].data(), m_rowptr[m].size() * sizeof(uint64_t));
       if (cols && cols[m]) memcpy(cols[m], m_col[m].data(), m_col[m].size() * sizeof(uint64_t));
@@ -514,6 +581,7 @@ struct MarlinIndex : IndexBase {
                 B2M_ERR_MISSING_RNG, "unsupported rng kind %d", rng->kind);
     if (const char* e = getenv("B2M_NTT_SHARE_MIN_LOG")) ntt_share_min_log = atoi(e);
     Timer tm(cx);
+    HostStager<Fr> stager(cx, copy_stream);  // (used by a host-resident index only)
     size_t t_all = tm.begin("Marlin::Prover");
     ZkSource<b2m_rng> zk(rng);
     const Fr* tw = ntt.table.tw;
@@ -695,15 +763,31 @@ struct MarlinIndex : IndexBase {
       const Fr* pvc = ieval[4].p;
       Fr* pb = b_ev.p; Fr* pf = f_ev.p;
       // b|_K = alpha beta - alpha row - beta col + row_col = (beta - row)(alpha - col)
-      ew(cx, K, [=] __device__(size_t i) {
-        Fr d = (beta - ld_fr(prow + i)) * (alpha - ld_fr(pcol + i));
-        st_fr(pb + i, d);
-        st_fr(pf + i, d);
-      });
-      batch_inverse<Fr>(cx, f_ev.p, K);
-      ew(cx, K, [=] __device__(size_t i) {
-        st_fr(pf + i, ld_fr(pf + i) * (ea_v * ld_fr(pva + i) + eb_v * ld_fr(pvb + i) + ec_v * ld_fr(pvc + i)));
-      });
+      if (!hvec) {
+        ew(cx, K, [=] __device__(size_t i) {
+          Fr d = (beta - ld_fr(prow + i)) * (alpha - ld_fr(pcol + i));
+          st_fr(pb + i, d);
+          st_fr(pf + i, d);
+        });
+        batch_inverse<Fr>(cx, f_ev.p, K);
+        ew(cx, K, [=] __device__(size_t i) {
+          st_fr(pf + i, ld_fr(pf + i) * (ea_v * ld_fr(pva + i) + eb_v * ld_fr(pvb + i) + ec_v * ld_fr(pvc + i)));
+        });
+      } else {  // the same two passes over row, col and over a_val, b_val, c_val streamed from pinned host memory
+        const Fr* ab[2] = {vec(6), vec(7)};
+        stager.stream("index_r3_denominators", ab, 2, K, [&](const Fr* slot, size_t stride, size_t at, size_t m) {
+          index_r3_denominators_kernel<Fr><<<div_up(m, 256), 256, 0, cx.stream>>>(slot, slot + stride, m, alpha, beta, pb + at, pf + at);
+          B2M_CHECK_LAUNCH();
+          cx.launches++;
+        });
+        batch_inverse<Fr>(cx, f_ev.p, K);
+        const Fr* abc[3] = {vec(8), vec(9), vec(10)};
+        stager.stream("index_r3_f", abc, 3, K, [&](const Fr* slot, size_t stride, size_t at, size_t m) {
+          index_r3_f_kernel<Fr><<<div_up(m, 256), 256, 0, cx.stream>>>(slot, stride, m, ea_v, eb_v, ec_v, pf + at);
+          B2M_CHECK_LAUNCH();
+          cx.launches++;
+        });
+      }
       run_ntt_group({NttJob{nullptr, 0, b_ev.p, b_poly.p, log_k, true}, NttJob{nullptr, 0, f_ev.p, f_poly.p, log_k, true}});
       // b * f on 2|K|; h_2 = (a - b f) / v_K = -(b f)[|K| ..]
       DBuf<Fr> eb2(cx, 2 * K), ef2(cx, 2 * K), bf(cx, 2 * K);
@@ -776,7 +860,7 @@ struct MarlinIndex : IndexBase {
     points[1].z = gamma;  // labels g_2, inner_sumcheck
     points[1].lcs = {Lc{{{&o_g2, one}}, s_g2.p + 1},
                      Lc{{{&ip[2], ci_a}, {&ip[3], ci_b}, {&ip[4], ci_c}, {&ip[0], ci_row}, {&ip[1], ci_col}, {&ip[5], ci_rc}, {&o_h2, ci_h2}}}};
-    std::vector<Opening<Fr, Fq>> openings = pc_open(srs, msm, pc, xi, points);
+    std::vector<Opening<Fr, Fq>> openings = pc_open(srs, msm, pc, xi, points, hvec ? &stager : nullptr);
     tm.end(t_op);
 
     // ---- Proof::new + CanonicalSerialize [reference data_structures.rs:100-126; SURVEY.md A.3] -----------
@@ -807,6 +891,10 @@ struct MarlinIndex : IndexBase {
     zk.commit_position();
     tm.end(t_all);
     timings_json = tm.json();
+    if (hvec) {  // the copy engine's share: bytes of index vectors streamed and the time their copies took
+      timings_json.pop_back();
+      timings_json += fmt(", \"IndexStream::H2D\": %.4f, \"IndexStream::bytes\": %zu}", stager.copy_ms(), stager.bytes);
+    }
   }
 
   // DensePolynomial::rand(3|H| - 1, zk_rng): on the device when the rng is a ChaCha stream position (attempts are 8-word

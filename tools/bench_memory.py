@@ -4,11 +4,14 @@ For each configuration -- log2 of the constraints, curve, PC, and either a devic
 (window tables, pass cap) -- runs universal_setup -> index -> prove (warm-up, then timed proves) on a DummyCircuit with
 |K| = 4|H|, and prints one JSON line: ms per proof, the layout (c, T, pass cap), the byte model's figures and budget, the device
 pool's high-water mark over setup + index + prove, and GPU verification of the proof (true) and of a wrong public input (false).
-A key the model refuses is reported with the refusal's message.  The card's name and power limit are read in the same run.
+It also records where the index keeps its twelve |K|-vectors ("device", or "host": pinned, streamed to every proof), the pinned
+bytes, and per proof the bytes streamed, the copy engine's time on them and the host-to-device rate this gives.  A key the
+model refuses is reported with the refusal's message.  The card's name and power limit are read in the same run.
 
     python tools/bench_memory.py --log-n 20 --tables 0 4 2 1          # one line per forced table count (0: the planned layout)
     python tools/bench_memory.py --log-n 22 --pc sonic_kzg10
     python tools/bench_memory.py --log-n 23 --limit-gb 70
+    python tools/bench_memory.py --log-n 20 --index-host                 # host-resident index at a size that fits the device
 """
 import argparse
 import json
@@ -38,6 +41,9 @@ def run(args, tables, cap):
            "card": card()}
     if cap:
         os.environ["B2M_MSM_MAX_PAIRS"] = str(cap)
+    if args.index_host:
+        os.environ["B2M_INDEX_HOST"] = "1"
+        rec["forced_index_host"] = True
     try:
         m = api.Marlin(args.curve, args.pc, ctx=ctx)
         a, b = 0x1234567890abcdef1234567890abcdef, 0xfedcba0987654321fedcba0987654321
@@ -57,16 +63,24 @@ def run(args, tables, cap):
         try:
             pk = m.index(srs, circ)
             rec["setup_index_s"] = round(time.time() - t0, 2)
+            rec["residency"], rec["pinned_bytes"] = pk.residency, pk.host_bytes
             try:
                 m.stage(pk, circ)
                 zk = api.ZkRng.test_rng()
                 for _ in range(args.warmup):
                     m.prove(pk, None, zk)
-                ms = []
+                ms, h2d = [], []
                 for _ in range(args.steps):
                     m.prove(pk, None, zk)
-                    ms.append(pk.timings()["Marlin::Prover"])
+                    t = pk.timings()
+                    ms.append(t["Marlin::Prover"])
+                    if "IndexStream::H2D" in t:
+                        h2d.append(t["IndexStream::H2D"])
+                        rec["streamed_bytes_per_proof"] = int(t["IndexStream::bytes"])
                 rec["ms_per_proof"] = round(sum(ms) / len(ms), 2)
+                if h2d:
+                    rec["h2d_ms_per_proof"] = round(sum(h2d) / len(h2d), 2)
+                    rec["h2d_gb_per_s"] = round(rec["streamed_bytes_per_proof"] / (rec["h2d_ms_per_proof"] * 1e6), 2)
                 rec["ms_min_max"] = [round(min(ms), 2), round(max(ms), 2)]
                 rec["pool_peak"] = ctx.memory()["peak"]
                 proof = m.prove(pk, circ, api.ZkRng.test_rng())
@@ -86,6 +100,7 @@ def run(args, tables, cap):
     except _lib.B2MError as e:
         rec["error"] = str(e)
     finally:
+        os.environ.pop("B2M_INDEX_HOST", None)
         ctx.close()
     return rec
 
@@ -98,6 +113,7 @@ def main():
     ap.add_argument("--limit-gb", type=float, default=0.0, help="device-memory limit of the context (0: free device memory)")
     ap.add_argument("--tables", type=int, nargs="*", default=[0], help="forced window tables, one run each (0: the planned layout)")
     ap.add_argument("--max-pairs", type=int, default=0, help="forced MSM pass cap (0: the planned one)")
+    ap.add_argument("--index-host", action="store_true", help="force a host-resident index (B2M_INDEX_HOST=1)")
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--out", default=None, help="also append the JSON lines to this file")
