@@ -22,6 +22,7 @@ def lib():
         vp, sz, ci = ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int
         L.cport_msm.argtypes = [ci, vp, vp, sz, vp, ci]
         L.cport_fft.argtypes = [ci, vp, ctypes.c_uint, ci, ci]
+        L.cport_coset_fft.argtypes = [ci, vp, ctypes.c_uint, ci, ci]
         L.cport_gen_bases.argtypes = [ci, vp, sz, vp]
         L.cport_max_threads.restype = ci
         L.cport_set_skip_index_commit.argtypes = [ci]
@@ -109,6 +110,16 @@ def fft(curve_name, data_limbs, inverse=False, threads=0):
     log_n = n.bit_length() - 1
     assert 1 << log_n == n and data_limbs.flags["C_CONTIGUOUS"]
     lib().cport_fft(CURVE_ID[curve_name], _ptr(data_limbs), log_n, 1 if inverse else 0, threads)
+    return data_limbs
+
+
+def coset_fft(curve_name, data_limbs, inverse=False, threads=0):
+    """in-place coset FFT (ark-poly `coset_fft` / `coset_ifft`, offset = the field's multiplicative generator) of (2^k, 4)
+    uint64 Montgomery Fr limbs."""
+    n = len(data_limbs)
+    log_n = n.bit_length() - 1
+    assert 1 << log_n == n and data_limbs.flags["C_CONTIGUOUS"] and data_limbs.dtype == np.uint64
+    lib().cport_coset_fft(CURVE_ID[curve_name], _ptr(data_limbs), log_n, 1 if inverse else 0, threads)
     return data_limbs
 
 

@@ -38,4 +38,35 @@ int cport_fft(int curve, u64* data, unsigned log_n, int inverse, int threads) {
   return 0;
 }
 
+/* ark-poly `coset_fft` / `coset_ifft` over the coset g H, g the field's multiplicative generator:
+ * forward data[i] *= g^i then the FFT; inverse the inverse FFT then data[i] *= g^-i. */
+static void fr_coset_scale(f4_t* a, size_t n, u64 gen, int inverse, const f4_ctx* c, int threads) {
+  f4_t g = {{gen, 0, 0, 0}}; f4_to_mont(&g, &g, c);
+  if (inverse) f4_inv(&g, &g, c);
+  #pragma omp parallel num_threads(threads)
+  {
+    int nt = 1, id = 0;
+#ifdef _OPENMP
+    nt = omp_get_num_threads(); id = omp_get_thread_num();
+#endif
+    size_t lo = n * id / nt, hi = n * (id + 1) / nt;
+    if (lo < hi) {
+      u64 e[1] = {lo}; f4_t cur; f4_pow(&cur, &g, e, 1, c);
+      for (size_t i = lo; i < hi; i++) { f4_mul(&a[i], &a[i], &cur, c); f4_mul(&cur, &cur, &g, c); }
+    }
+  }
+}
+int cport_coset_fft(int curve, u64* data, unsigned log_n, int inverse, int threads) {
+  init_all();
+  if (threads <= 0) threads = max_threads();
+  const f4_ctx* c = curve == 0 ? &BLS_FR : &BN_FR;
+  const u64 gen = curve == 0 ? BLS_FR_GEN : BN_FR_GEN;
+  const int s = curve == 0 ? BLS_FR_S : BN_FR_S;
+  size_t n = (size_t)1 << log_n;
+  if (!inverse) fr_coset_scale((f4_t*)data, n, gen, 0, c, threads);
+  fr_fft((f4_t*)data, (int)log_n, inverse, c, gen, s, threads);
+  if (inverse) fr_coset_scale((f4_t*)data, n, gen, 1, c, threads);
+  return 0;
+}
+
 int cport_max_threads(void) { return max_threads(); }

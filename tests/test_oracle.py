@@ -191,6 +191,26 @@ def test_cport_matches_python_oracle():
             assert util.fr_from_mont_limbs(curve, buf) == vals
 
 
+@pytest.mark.parametrize("curve", [BLS12_381, BN254], ids=lambda c: c.name)
+@pytest.mark.parametrize("log_n", [0, 1, 5, 10])
+def test_cport_coset_fft_matches_python_oracle(curve, log_n):
+    """cport.coset_fft (the checker of the GPU's coset NTTs at sizes Python cannot reach) equals Domain.coset_fft and
+    coset_ifft, with 0, 1 and p - 1 among the inputs."""
+    f = curve.fr
+    rnd = random.Random(40 + log_n)
+    n = 1 << log_n
+    d = P.Domain(f, n)
+    vals = [rnd.randrange(f.p) for _ in range(n)]
+    for i, v in zip(range(n), (f.p - 1, 0, 1)):
+        vals[-1 - i] = v
+    buf = util.fr_to_mont_limbs(curve, vals)
+    cport.coset_fft(curve.name, buf)
+    assert util.fr_from_mont_limbs(curve, buf) == d.coset_fft(vals)
+    buf = util.fr_to_mont_limbs(curve, vals)
+    cport.coset_fft(curve.name, buf, inverse=True)
+    assert util.fr_from_mont_limbs(curve, buf) == d.coset_ifft(vals)
+
+
 @pytest.mark.parametrize("case", [c["name"] for c in load_golden()["cases"]] if os.path.exists(os.path.join(GOLDEN, "marlin_proofs.json")) else [])
 def test_cpp_prover_reproduces_golden(case):
     """oracle/cport/prover.cpp (the C++ restatement of the reference prover used as CPU baseline) is byte-identical
