@@ -56,6 +56,7 @@ pub const B2M_ERR_SERIALIZATION: c_int = 11;
 pub const B2M_ERR_MEMORY_LIMIT: c_int = 12;
 pub const B2M_CURVE_BLS12_381: c_int = 0;
 pub const B2M_CURVE_BN254: c_int = 1;
+pub const B2M_CURVE_BLS12_377: c_int = 2;
 pub const B2M_PC_MARLIN_KZG10: c_int = 0;
 pub const B2M_PC_SONIC_KZG10: c_int = 1;
 

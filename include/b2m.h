@@ -44,7 +44,7 @@ enum {
   B2M_ERR_MEMORY_LIMIT = 12             /* the byte model of a key or an index exceeds the device-memory budget (b2m_ctx_set_memory_limit) */
 };
 
-enum { B2M_CURVE_BLS12_381 = 0, B2M_CURVE_BN254 = 1 };
+enum { B2M_CURVE_BLS12_381 = 0, B2M_CURVE_BN254 = 1, B2M_CURVE_BLS12_377 = 2 };
 enum { B2M_PC_MARLIN_KZG10 = 0, B2M_PC_SONIC_KZG10 = 1 };
 /* stream ciphers behind `RngCore`: rand 0.8 StdRng (= ChaCha12, `ark_std::test_rng`) and
  * rand_chacha::ChaChaRng (= ChaCha20). */

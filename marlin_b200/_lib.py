@@ -10,6 +10,7 @@ LIB_PATH = os.path.join(_HERE, "libb2m.so")
 
 CURVE_BLS12_381 = 0
 CURVE_BN254 = 1
+CURVE_BLS12_377 = 2
 PC_MARLIN_KZG10 = 0
 PC_SONIC_KZG10 = 1
 RNG_CHACHA8, RNG_CHACHA12, RNG_CHACHA20 = 8, 12, 20
@@ -20,7 +21,7 @@ POINT_REASONS = {1: "both flag bits set", 2: "x is not below the field modulus",
                  5: "y is not below the field modulus"}
 
 # (Fr u64 limbs, Fq u64 limbs) per curve id
-LIMBS = {CURVE_BLS12_381: (4, 6), CURVE_BN254: (4, 4)}
+LIMBS = {CURVE_BLS12_381: (4, 6), CURVE_BN254: (4, 4), CURVE_BLS12_377: (4, 6)}
 
 
 class B2MError(RuntimeError):

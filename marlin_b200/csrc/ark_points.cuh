@@ -1,5 +1,5 @@
 // Batch conversion of ark-serialize G1 / G2 points and Fr elements on the GPU (the SRS and index-key loaders:
-// b2m_g1_decode_ark, b2m_g2_decode_ark, b2m_g1_to_compressed, b2m_fr_decode_ark, b2m_fr_to_canonical).  Definitions in ark_points_impl.cuh, instantiated per curve by inst_ark_{bls,bn}.cu.
+// b2m_g1_decode_ark, b2m_g2_decode_ark, b2m_g1_to_compressed, b2m_fr_decode_ark, b2m_fr_to_canonical).  Definitions in ark_points_impl.cuh, instantiated per curve by inst_ark_{bls,bn,bls377}.cu.
 #pragma once
 #include "common.cuh"
 #include "field.cuh"

@@ -106,9 +106,7 @@ int b2m_ntt(b2m_ctx* ctx, int curve, uint64_t* data, unsigned log_n, int inverse
   return guard([&] {
     B2M_REQUIRE(ctx && data, B2M_ERR_INVALID_ARG, "null argument");
     ctx->cx.use();
-    if (curve == B2M_CURVE_BLS12_381) ctx->ntt_bls().run_host(data, log_n, inverse != 0, coset != 0);
-    else if (curve == B2M_CURVE_BN254) ctx->ntt_bn().run_host(data, log_n, inverse != 0, coset != 0);
-    else throw Error(B2M_ERR_INVALID_ARG, "unknown curve id");
+    with_curve(curve, [&](auto t) { ctx->ntt<typename decltype(t)::Fr>().run_host(data, log_n, inverse != 0, coset != 0); });
   });
 }
 
@@ -116,7 +114,7 @@ int b2m_srs_create_layout(b2m_ctx* ctx, int curve, const uint64_t* powers_of_g, 
                           const uint64_t* gamma_indices, size_t n_gamma, int window_bits, int window_tables, b2m_srs** out) {
   return guard([&] {
     B2M_REQUIRE(ctx && powers_of_g && out, B2M_ERR_INVALID_ARG, "null argument");
-    B2M_REQUIRE(curve == B2M_CURVE_BLS12_381 || curve == B2M_CURVE_BN254, B2M_ERR_INVALID_ARG, "unknown curve id");
+    require_curve(curve);
     B2M_REQUIRE(window_tables >= 0, B2M_ERR_INVALID_ARG, "window_tables %d < 0", window_tables);
     ctx->cx.use();
     *out = new b2m_srs(ctx, curve, powers_of_g, n_g, powers_of_gamma_g, gamma_indices, n_gamma, window_bits, window_tables);
@@ -156,8 +154,7 @@ int b2m_srs_msm(b2m_srs* srs, size_t base_off, const uint64_t* scalars, size_t n
   return guard([&] {
     B2M_REQUIRE(srs && out_xy && (scalars || n == 0), B2M_ERR_INVALID_ARG, "null argument");
     srs->ctx->cx.use();
-    if (srs->curve == B2M_CURVE_BLS12_381) srs->bls->run_host(base_off, scalars, n, out_xy, out_is_inf);
-    else srs->bn->run_host(base_off, scalars, n, out_xy, out_is_inf);
+    with_curve(srs->curve, [&](auto t) { srs->msm<typename decltype(t)::Fr>()->run_host(base_off, scalars, n, out_xy, out_is_inf); });
   });
 }
 
@@ -195,9 +192,11 @@ int b2m_g1_powers(b2m_ctx* ctx, int curve, const uint64_t* g_xy, const uint64_t*
   return guard([&] {
     B2M_REQUIRE(ctx && g_xy && beta && out_powers_xy, B2M_ERR_INVALID_ARG, "null argument");
     ctx->cx.use();
-    if (curve == B2M_CURVE_BLS12_381) Msm<FrBls, FqBls>::g1_powers_host(ctx->cx, g_xy, beta, n, out_powers_xy);
-    else if (curve == B2M_CURVE_BN254) Msm<FrBn, FqBn>::g1_powers_host(ctx->cx, g_xy, beta, n, out_powers_xy);
-    else throw Error(B2M_ERR_INVALID_ARG, "unknown curve id");
+    with_curve(curve, [&](auto t) {
+      using Fr = typename decltype(t)::Fr;
+      using Fq = typename decltype(t)::Fq;
+      Msm<Fr, Fq>::g1_powers_host(ctx->cx, g_xy, beta, n, out_powers_xy);
+    });
   });
 }
 
@@ -205,9 +204,11 @@ int b2m_fixed_base_msm(b2m_ctx* ctx, int curve, const uint64_t* g_xy, const uint
   return guard([&] {
     B2M_REQUIRE(ctx && g_xy && (scalars || n == 0) && (out_xy || n == 0), B2M_ERR_INVALID_ARG, "null argument");
     ctx->cx.use();
-    if (curve == B2M_CURVE_BLS12_381) Msm<FrBls, FqBls>::fixed_base_host(ctx->cx, g_xy, scalars, nullptr, 0, n, out_xy);
-    else if (curve == B2M_CURVE_BN254) Msm<FrBn, FqBn>::fixed_base_host(ctx->cx, g_xy, scalars, nullptr, 0, n, out_xy);
-    else throw Error(B2M_ERR_INVALID_ARG, "unknown curve id");
+    with_curve(curve, [&](auto t) {
+      using Fr = typename decltype(t)::Fr;
+      using Fq = typename decltype(t)::Fq;
+      Msm<Fr, Fq>::fixed_base_host(ctx->cx, g_xy, scalars, nullptr, 0, n, out_xy);
+    });
   });
 }
 
@@ -216,31 +217,35 @@ int b2m_srs_export_g1(b2m_srs* srs, size_t first, size_t n, uint8_t* out) {
     B2M_REQUIRE(srs && (out || n == 0), B2M_ERR_INVALID_ARG, "null argument");
     B2M_REQUIRE(first + n <= srs->n_g, B2M_ERR_INVALID_ARG, "powers [%zu, %zu) of %zu", first, first + n, srs->n_g);
     srs->ctx->cx.use();
-    if (srs->curve == B2M_CURVE_BLS12_381) {
-      B2M_REQUIRE(srs->bls->tab_world == 1, B2M_ERR_UNSUPPORTED, "export from a sharded key");
-      Msm<FrBls, FqBls>::g1_to_bytes(srs->ctx->cx, srs->bls->tables.p + first, nullptr, n, out);
-    } else {
-      B2M_REQUIRE(srs->bn->tab_world == 1, B2M_ERR_UNSUPPORTED, "export from a sharded key");
-      Msm<FrBn, FqBn>::g1_to_bytes(srs->ctx->cx, srs->bn->tables.p + first, nullptr, n, out);
-    }
+    with_curve(srs->curve, [&](auto t) {
+      using Fr = typename decltype(t)::Fr;
+      using Fq = typename decltype(t)::Fq;
+      const auto& m = srs->msm<Fr>();
+      B2M_REQUIRE(m->tab_world == 1, B2M_ERR_UNSUPPORTED, "export from a sharded key");
+      Msm<Fr, Fq>::g1_to_bytes(srs->ctx->cx, m->tables.p + first, nullptr, n, out);
+    });
   });
 }
 int b2m_g1_to_uncompressed(b2m_ctx* ctx, int curve, const uint64_t* points_xy, size_t n, uint8_t* out) {
   return guard([&] {
     B2M_REQUIRE(ctx && ((points_xy && out) || n == 0), B2M_ERR_INVALID_ARG, "null argument");
     ctx->cx.use();
-    if (curve == B2M_CURVE_BLS12_381) Msm<FrBls, FqBls>::g1_to_bytes(ctx->cx, nullptr, points_xy, n, out);
-    else if (curve == B2M_CURVE_BN254) Msm<FrBn, FqBn>::g1_to_bytes(ctx->cx, nullptr, points_xy, n, out);
-    else throw Error(B2M_ERR_INVALID_ARG, "unknown curve id");
+    with_curve(curve, [&](auto t) {
+      using Fr = typename decltype(t)::Fr;
+      using Fq = typename decltype(t)::Fq;
+      Msm<Fr, Fq>::g1_to_bytes(ctx->cx, nullptr, points_xy, n, out);
+    });
   });
 }
 int b2m_g1_from_uncompressed(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, uint64_t* out_xy) {
   return guard([&] {
     B2M_REQUIRE(ctx && ((bytes && out_xy) || n == 0), B2M_ERR_INVALID_ARG, "null argument");
     ctx->cx.use();
-    if (curve == B2M_CURVE_BLS12_381) Msm<FrBls, FqBls>::g1_from_bytes(ctx->cx, bytes, n, out_xy);
-    else if (curve == B2M_CURVE_BN254) Msm<FrBn, FqBn>::g1_from_bytes(ctx->cx, bytes, n, out_xy);
-    else throw Error(B2M_ERR_INVALID_ARG, "unknown curve id");
+    with_curve(curve, [&](auto t) {
+      using Fr = typename decltype(t)::Fr;
+      using Fq = typename decltype(t)::Fq;
+      Msm<Fr, Fq>::g1_from_bytes(ctx->cx, bytes, n, out_xy);
+    });
   });
 }
 
@@ -253,11 +258,11 @@ int b2m_g1_decode_ark(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, i
                       int* bad_reason) {
   return guard([&] {
     B2M_REQUIRE(ctx && ((bytes && out_xy) || n == 0), B2M_ERR_INVALID_ARG, "null argument");
-    B2M_REQUIRE(curve == B2M_CURVE_BLS12_381 || curve == B2M_CURVE_BN254, B2M_ERR_INVALID_ARG, "unknown curve id");
+    require_curve(curve);
     ctx->cx.use();
-    const ArkBad bad = n == 0 ? ArkBad{0, G1_OK}
-                     : curve == B2M_CURVE_BLS12_381 ? g1_decode_ark<FqBls>(ctx->cx, bytes, n, compressed != 0, out_xy)
-                                                    : g1_decode_ark<FqBn>(ctx->cx, bytes, n, compressed != 0, out_xy);
+    const ArkBad bad = n == 0 ? ArkBad{0, G1_OK} : with_curve(curve, [&](auto t) {
+      return g1_decode_ark<typename decltype(t)::Fq>(ctx->cx, bytes, n, compressed != 0, out_xy);
+    });
     if (ark_fail(bad, bad_index, bad_reason) != B2M_OK)
       throw Error(B2M_ERR_SERIALIZATION, fmt("G1 point %zu: %s", bad.index, point_status_name(bad.reason)));
   });
@@ -266,11 +271,11 @@ int b2m_g2_decode_ark(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, i
                       int* bad_reason) {
   return guard([&] {
     B2M_REQUIRE(ctx && ((bytes && out_uncompressed) || n == 0), B2M_ERR_INVALID_ARG, "null argument");
-    B2M_REQUIRE(curve == B2M_CURVE_BLS12_381 || curve == B2M_CURVE_BN254, B2M_ERR_INVALID_ARG, "unknown curve id");
+    require_curve(curve);
     ctx->cx.use();
-    const ArkBad bad = n == 0 ? ArkBad{0, G1_OK}
-                     : curve == B2M_CURVE_BLS12_381 ? g2_decode_ark<FqBls>(ctx->cx, bytes, n, compressed != 0, out_uncompressed)
-                                                    : g2_decode_ark<FqBn>(ctx->cx, bytes, n, compressed != 0, out_uncompressed);
+    const ArkBad bad = n == 0 ? ArkBad{0, G1_OK} : with_curve(curve, [&](auto t) {
+      return g2_decode_ark<typename decltype(t)::Fq>(ctx->cx, bytes, n, compressed != 0, out_uncompressed);
+    });
     if (ark_fail(bad, bad_index, bad_reason) != B2M_OK)
       throw Error(B2M_ERR_SERIALIZATION, fmt("G2 point %zu: %s", bad.index, point_status_name(bad.reason)));
   });
@@ -280,19 +285,16 @@ int b2m_g1_to_compressed(b2m_ctx* ctx, int curve, const uint64_t* points_xy, siz
     B2M_REQUIRE(ctx && ((points_xy && out) || n == 0), B2M_ERR_INVALID_ARG, "null argument");
     ctx->cx.use();
     if (n == 0) return;
-    if (curve == B2M_CURVE_BLS12_381) g1_to_compressed<FqBls>(ctx->cx, points_xy, n, out);
-    else if (curve == B2M_CURVE_BN254) g1_to_compressed<FqBn>(ctx->cx, points_xy, n, out);
-    else throw Error(B2M_ERR_INVALID_ARG, "unknown curve id");
+    with_curve(curve, [&](auto t) { g1_to_compressed<typename decltype(t)::Fq>(ctx->cx, points_xy, n, out); });
   });
 }
 int b2m_g2_to_compressed(int curve, const uint8_t* uncompressed, size_t n, uint8_t* out) {
   return guard([&] {
     B2M_REQUIRE((uncompressed && out) || n == 0, B2M_ERR_INVALID_ARG, "null argument");
-    if (curve == B2M_CURVE_BLS12_381)
-      for (size_t i = 0; i < n; i++) g2_compress<FqBls>(uncompressed + i * 4 * FqBls::N * 4, out + i * 2 * FqBls::N * 4);
-    else if (curve == B2M_CURVE_BN254)
-      for (size_t i = 0; i < n; i++) g2_compress<FqBn>(uncompressed + i * 4 * FqBn::N * 4, out + i * 2 * FqBn::N * 4);
-    else throw Error(B2M_ERR_INVALID_ARG, "unknown curve id");
+    with_curve(curve, [&](auto t) {
+      using Fq = typename decltype(t)::Fq;
+      for (size_t i = 0; i < n; i++) g2_compress<Fq>(uncompressed + i * 4 * Fq::N * 4, out + i * 2 * Fq::N * 4);
+    });
   });
 }
 
@@ -317,22 +319,20 @@ extern "C" {
 int b2m_fr_decode_ark(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, uint64_t* out_limbs, size_t* bad_index) {
   return guard([&] {
     B2M_REQUIRE(ctx && ((bytes && out_limbs) || n == 0), B2M_ERR_INVALID_ARG, "null argument");
-    B2M_REQUIRE(curve == B2M_CURVE_BLS12_381 || curve == B2M_CURVE_BN254, B2M_ERR_INVALID_ARG, "unknown curve id");
+    require_curve(curve);
     if (bad_index) *bad_index = n;
     if (n == 0) return;
     ctx->cx.use();
-    if (curve == B2M_CURVE_BLS12_381) fr_decode_host<FrBls>(ctx->cx, bytes, n, out_limbs, bad_index);
-    else fr_decode_host<FrBn>(ctx->cx, bytes, n, out_limbs, bad_index);
+    with_curve(curve, [&](auto t) { fr_decode_host<typename decltype(t)::Fr>(ctx->cx, bytes, n, out_limbs, bad_index); });
   });
 }
 int b2m_fr_to_canonical(b2m_ctx* ctx, int curve, const uint64_t* limbs, size_t n, uint8_t* out) {
   return guard([&] {
     B2M_REQUIRE(ctx && ((limbs && out) || n == 0), B2M_ERR_INVALID_ARG, "null argument");
-    B2M_REQUIRE(curve == B2M_CURVE_BLS12_381 || curve == B2M_CURVE_BN254, B2M_ERR_INVALID_ARG, "unknown curve id");
+    require_curve(curve);
     if (n == 0) return;
     ctx->cx.use();
-    if (curve == B2M_CURVE_BLS12_381) fr_encode_host<FrBls>(ctx->cx, limbs, n, out);
-    else fr_encode_host<FrBn>(ctx->cx, limbs, n, out);
+    with_curve(curve, [&](auto t) { fr_encode_host<typename decltype(t)::Fr>(ctx->cx, limbs, n, out); });
   });
 }
 
@@ -390,9 +390,7 @@ extern "C" {
 int b2m_domain_ark(int curve, unsigned log_size, uint8_t* out) {
   return guard([&] {
     B2M_REQUIRE(out != nullptr, B2M_ERR_INVALID_ARG, "null argument");
-    if (curve == B2M_CURVE_BLS12_381) domain_ark_impl<FrBls>(log_size, out);
-    else if (curve == B2M_CURVE_BN254) domain_ark_impl<FrBn>(log_size, out);
-    else throw Error(B2M_ERR_INVALID_ARG, "unknown curve id");
+    with_curve(curve, [&](auto t) { domain_ark_impl<typename decltype(t)::Fr>(log_size, out); });
   });
 }
 
@@ -406,6 +404,17 @@ static const char* const G2_GEN_BLS[4] = {
 static const char* const G2_GEN_BN[4] = {
     "1800deef121f1e76426a00665e5c4479674322d4f75edadd46debd5cd992f6ed", "198e9393920d483a7260bfb731fb5d25f1aa493335a9e71297e485b7aef312c2",
     "12c85ea5db8c6deb4aab71808dcb408fe3d1e7690c43d37b4ce6cc0166fa7daa", "090689d0585ff075ec9e99ad690c3395bc4b313370b38ef355acdadcd122975b"};
+static const char* const G2_GEN_BLS377[4] = {  // ark-bls12-377's G2 generator
+    "018480be71c785fec89630a2a3841d01c565f071203e50317ea501f557db6b9b71889f52bb53540274e3e48f7c005196",
+    "00ea6040e700403170dc5a51b1b140d5532777ee6651cecbe7223ece0799c9de5cf89984bff76fe6b26bfefa6ea16afe",
+    "00690d665d446f7bd960736bcbb2efb4de03ed7274b49a58e458c282f832d204f2cf88886d8c7c2ef094094409fd4ddf",
+    "00f8169fd28355189e549da3151a70aa61ef11ac3d591bf12463b01acee304c24279b83f5e52270bd9a1cdd185eb8f93"};
+template <class Fq>
+static const char* const* g2_generator_hex() {
+  if constexpr (std::is_same<Fq, FqBls>::value) return G2_GEN_BLS;
+  else if constexpr (std::is_same<Fq, FqBn>::value) return G2_GEN_BN;
+  else return G2_GEN_BLS377;
+}
 
 template <class Fq>
 static Fq fq_from_hex(const char* hex) {
@@ -444,13 +453,19 @@ extern "C" {
 int b2m_g2_scalar_muls(int curve, const uint8_t* h_uncompressed, const uint64_t* scalars, size_t n, uint8_t* out) {
   return guard([&] {
     B2M_REQUIRE((scalars && out) || n == 0, B2M_ERR_INVALID_ARG, "null argument");
-    if (curve == B2M_CURVE_BLS12_381) g2_scalar_muls_impl<FqBls>(G2_GEN_BLS, h_uncompressed, scalars, n, out);
-    else if (curve == B2M_CURVE_BN254) g2_scalar_muls_impl<FqBn>(G2_GEN_BN, h_uncompressed, scalars, n, out);
-    else throw Error(B2M_ERR_INVALID_ARG, "unknown curve id");
+    with_curve(curve, [&](auto t) {
+      using Fq = typename decltype(t)::Fq;
+      g2_scalar_muls_impl<Fq>(g2_generator_hex<Fq>(), h_uncompressed, scalars, n, out);
+    });
   });
 }
 
 // ---- Level 1 ----------------------------------------------------------------------------------
+}  // extern "C"
+static decltype(&pc_open_combinations_bls) pc_open_combinations_of(int curve) {
+  return curve == B2M_CURVE_BLS12_381 ? pc_open_combinations_bls : curve == B2M_CURVE_BN254 ? pc_open_combinations_bn : pc_open_combinations_bls377;
+}
+extern "C" {
 int b2m_pc_commit(b2m_srs* srs, int pc_variant, size_t n_polys, const uint64_t* const* coeffs, const size_t* n_coeffs,
                   const int64_t* degree_bounds, const int64_t* hiding_bounds, b2m_rng* rng, uint64_t* out_comm_xy,
                   uint64_t* out_shifted_xy, uint64_t* out_rand, uint64_t* out_shifted_rand, size_t rand_stride) {
@@ -463,12 +478,9 @@ int b2m_pc_commit(b2m_srs* srs, int pc_variant, size_t n_polys, const uint64_t* 
                     (rng->kind == B2M_RNG_CALLBACK && rng->next_u64 != nullptr),
                 B2M_ERR_MISSING_RNG, "unsupported rng kind");
     srs->ctx->cx.use();
-    if (srs->curve == B2M_CURVE_BLS12_381)
-      pc_commit_bls(srs, pc_variant, n_polys, coeffs, n_coeffs, degree_bounds, hiding_bounds, rng, out_comm_xy, out_shifted_xy, out_rand,
-                    out_shifted_rand, rand_stride);
-    else
-      pc_commit_bn(srs, pc_variant, n_polys, coeffs, n_coeffs, degree_bounds, hiding_bounds, rng, out_comm_xy, out_shifted_xy, out_rand,
-                   out_shifted_rand, rand_stride);
+    const auto commit = srs->curve == B2M_CURVE_BLS12_381 ? pc_commit_bls : srs->curve == B2M_CURVE_BN254 ? pc_commit_bn : pc_commit_bls377;
+    commit(srs, pc_variant, n_polys, coeffs, n_coeffs, degree_bounds, hiding_bounds, rng, out_comm_xy, out_shifted_xy, out_rand, out_shifted_rand,
+           rand_stride);
   });
 }
 
@@ -484,7 +496,6 @@ int b2m_pc_open(b2m_srs* srs, int pc_variant, size_t n_polys, const uint64_t* co
     srs->ctx->cx.use();
     // open_combinations with one coefficient-one combination per polynomial, all queried at the one point; null rands
     // give empty randomness
-    const bool bls = srs->curve == B2M_CURVE_BLS12_381;
     std::vector<int> hiding(n_polys, 1);
     std::vector<size_t> term_off(n_polys + 1), lc(n_polys), at_point(n_polys, 0);
     std::vector<int64_t> poly(n_polys);
@@ -493,16 +504,11 @@ int b2m_pc_open(b2m_srs* srs, int pc_variant, size_t n_polys, const uint64_t* co
       term_off[i + 1] = i + 1;
       lc[i] = i;
       poly[i] = (int64_t)i;
-      memcpy(&ones[4 * i], bls ? FrBls::one().l : FrBn::one().l, 32);
+      with_curve(srs->curve, [&](auto t) { memcpy(&ones[4 * i], decltype(t)::Fr::one().l, 32); });
     }
-    if (bls)
-      pc_open_combinations_bls(srs, pc_variant, max_degree_bound, n_polys, coeffs, n_coeffs, degree_bounds, hiding.data(), rands, shifted_rands,
-                               rand_stride, n_polys, term_off.data(), poly.data(), ones.data(), n_polys, lc.data(), at_point.data(), 1, point,
-                               opening_challenge, out_w_xy, out_has_random_v, out_random_v);
-    else
-      pc_open_combinations_bn(srs, pc_variant, max_degree_bound, n_polys, coeffs, n_coeffs, degree_bounds, hiding.data(), rands, shifted_rands,
-                              rand_stride, n_polys, term_off.data(), poly.data(), ones.data(), n_polys, lc.data(), at_point.data(), 1, point,
-                              opening_challenge, out_w_xy, out_has_random_v, out_random_v);
+    pc_open_combinations_of(srs->curve)(srs, pc_variant, max_degree_bound, n_polys, coeffs, n_coeffs, degree_bounds, hiding.data(), rands,
+                                        shifted_rands, rand_stride, n_polys, term_off.data(), poly.data(), ones.data(), n_polys, lc.data(),
+                                        at_point.data(), 1, point, opening_challenge, out_w_xy, out_has_random_v, out_random_v);
   });
 }
 
@@ -548,8 +554,7 @@ int b2m_ck_shift_power(const b2m_ck* ck, uint64_t bound, uint64_t* out_xy) {
     b2m_srs* srs = ck->srs;
     srs->ctx->cx.use();
     const size_t slot = srs->n_g - 1 - bound;
-    if (srs->curve == B2M_CURVE_BLS12_381) srs->bls->read_power(slot, out_xy);
-    else srs->bn->read_power(slot, out_xy);
+    with_curve(srs->curve, [&](auto t) { srs->msm<typename decltype(t)::Fr>()->read_power(slot, out_xy); });
   });
 }
 
@@ -593,14 +598,9 @@ int b2m_ck_open_combinations(b2m_ck* ck, size_t n_polys, const uint64_t* const* 
     for (size_t q = 0; q < n_queries; q++) B2M_REQUIRE(query_point[q] < n_points, B2M_ERR_INVALID_ARG, "query %zu names point %zu of %zu", q, query_point[q], n_points);
     b2m_srs* srs = ck->srs;
     srs->ctx->cx.use();
-    if (srs->curve == B2M_CURVE_BLS12_381)
-      pc_open_combinations_bls(srs, ck->pc, ck->max_bound(), n_polys, coeffs, n_coeffs, degree_bounds, hiding, rands, shifted_rands, rand_stride, n_lcs,
-                               lc_term_off, lc_poly, lc_coeff, n_queries, query_lc, query_point, n_points, points, opening_challenge, out_w_xy,
-                               out_has_random_v, out_random_v);
-    else
-      pc_open_combinations_bn(srs, ck->pc, ck->max_bound(), n_polys, coeffs, n_coeffs, degree_bounds, hiding, rands, shifted_rands, rand_stride, n_lcs,
-                              lc_term_off, lc_poly, lc_coeff, n_queries, query_lc, query_point, n_points, points, opening_challenge, out_w_xy,
-                              out_has_random_v, out_random_v);
+    pc_open_combinations_of(srs->curve)(srs, ck->pc, ck->max_bound(), n_polys, coeffs, n_coeffs, degree_bounds, hiding, rands, shifted_rands,
+                                        rand_stride, n_lcs, lc_term_off, lc_poly, lc_coeff, n_queries, query_lc, query_point, n_points, points,
+                                        opening_challenge, out_w_xy, out_has_random_v, out_random_v);
   });
 }
 
@@ -618,10 +618,8 @@ int b2m_index_create(b2m_srs* srs, int pc_variant, size_t num_constraints, size_
     srs->ctx->cx.use();
     std::unique_ptr<b2m_index> idx(new b2m_index);
     idx->srs = srs;
-    if (srs->curve == B2M_CURVE_BLS12_381)
-      idx->impl.reset(make_index_bls(srs, pc_variant, num_constraints, num_variables, num_instance_variables, a, b, c));
-    else
-      idx->impl.reset(make_index_bn(srs, pc_variant, num_constraints, num_variables, num_instance_variables, a, b, c));
+    const auto make = srs->curve == B2M_CURVE_BLS12_381 ? make_index_bls : srs->curve == B2M_CURVE_BN254 ? make_index_bn : make_index_bls377;
+    idx->impl.reset(make(srs, pc_variant, num_constraints, num_variables, num_instance_variables, a, b, c));
     *out = idx.release();
     srs->children++;
   });
@@ -639,12 +637,9 @@ int b2m_index_load(b2m_srs* srs, int pc_variant, size_t num_constraints, size_t 
     srs->ctx->cx.use();
     std::unique_ptr<b2m_index> idx(new b2m_index);
     idx->srs = srs;
-    if (srs->curve == B2M_CURVE_BLS12_381)
-      idx->impl.reset(load_index_bls(srs, pc_variant, num_constraints, num_variables, num_instance_variables, num_non_zero, a, b, c, vectors,
-                                     vector_lens, index_comms_xy, check_commitments != 0, bad));
-    else
-      idx->impl.reset(load_index_bn(srs, pc_variant, num_constraints, num_variables, num_instance_variables, num_non_zero, a, b, c, vectors,
-                                    vector_lens, index_comms_xy, check_commitments != 0, bad));
+    const auto load = srs->curve == B2M_CURVE_BLS12_381 ? load_index_bls : srs->curve == B2M_CURVE_BN254 ? load_index_bn : load_index_bls377;
+    idx->impl.reset(load(srs, pc_variant, num_constraints, num_variables, num_instance_variables, num_non_zero, a, b, c, vectors, vector_lens,
+                         index_comms_xy, check_commitments != 0, bad));
     *out = idx.release();
     srs->children++;
   });
@@ -746,14 +741,15 @@ int b2m_vk_create(b2m_ctx* ctx, int curve, int pc_variant, size_t num_constraint
   return guard([&] {
     B2M_REQUIRE(ctx && index_comms_xy && g_xy && gamma_g_xy && h_bytes && beta_h_bytes && out && (n_bounds == 0 || (bounds && bound_points)),
                 B2M_ERR_INVALID_ARG, "null argument");
-    B2M_REQUIRE(curve == B2M_CURVE_BLS12_381 || curve == B2M_CURVE_BN254, B2M_ERR_INVALID_ARG, "unknown curve id");
+    require_curve(curve);
     B2M_REQUIRE(pc_variant == B2M_PC_MARLIN_KZG10 || pc_variant == B2M_PC_SONIC_KZG10, B2M_ERR_INVALID_ARG, "unknown PC variant");
     B2M_REQUIRE(ctx->cx.world <= 1, B2M_ERR_UNSUPPORTED, "verification on a multi-GPU context");
     ctx->cx.use();
     const VkArgs a{pc_variant, num_constraints, num_variables, num_non_zero, index_comms_xy, g_xy, gamma_g_xy, h_bytes, beta_h_bytes,
                    n_bounds, bounds, bound_points};
     std::unique_ptr<b2m_vk> vk(new b2m_vk{ctx, nullptr});
-    vk->impl.reset(curve == B2M_CURVE_BLS12_381 ? make_verifier_bls(ctx->cx, a) : make_verifier_bn(ctx->cx, a));
+    const auto make = curve == B2M_CURVE_BLS12_381 ? make_verifier_bls : curve == B2M_CURVE_BN254 ? make_verifier_bn : make_verifier_bls377;
+    vk->impl.reset(make(ctx->cx, a));
     *out = vk.release();
     ctx->children++;
   });

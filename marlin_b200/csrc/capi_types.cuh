@@ -3,6 +3,7 @@
 #include <cstdio>
 #include <memory>
 #include <string>
+#include <type_traits>
 
 #include "common.cuh"
 #include "msm.cuh"
@@ -34,6 +35,7 @@ struct b2m_ctx {
   bool dead = false;
   std::unique_ptr<b2m::Ntt<b2m::FrBls>> ntt_bls_;
   std::unique_ptr<b2m::Ntt<b2m::FrBn>> ntt_bn_;
+  std::unique_ptr<b2m::Ntt<b2m::FrBls377>> ntt_bls377_;
   explicit b2m_ctx(int device) : cx(device) {}
   b2m::Ntt<b2m::FrBls>& ntt_bls() {
     if (!ntt_bls_) ntt_bls_.reset(new b2m::Ntt<b2m::FrBls>(cx));
@@ -43,7 +45,39 @@ struct b2m_ctx {
     if (!ntt_bn_) ntt_bn_.reset(new b2m::Ntt<b2m::FrBn>(cx));
     return *ntt_bn_;
   }
+  b2m::Ntt<b2m::FrBls377>& ntt_bls377() {
+    if (!ntt_bls377_) ntt_bls377_.reset(new b2m::Ntt<b2m::FrBls377>(cx));
+    return *ntt_bls377_;
+  }
+  template <class Fr>
+  b2m::Ntt<Fr>& ntt() {
+    if constexpr (std::is_same<Fr, b2m::FrBls>::value) return ntt_bls();
+    else if constexpr (std::is_same<Fr, b2m::FrBn>::value) return ntt_bn();
+    else return ntt_bls377();
+  }
 };
+
+namespace b2m {
+template <class Fr_, class Fq_>
+struct CurveTypes {
+  using Fr = Fr_;
+  using Fq = Fq_;
+};
+// f(CurveTypes<Fr, Fq>{}) for a curve id (B2M_CURVE_*); an unknown id is B2M_ERR_INVALID_ARG
+template <class F>
+auto with_curve(int curve, F&& f) {
+  switch (curve) {
+    case B2M_CURVE_BLS12_381: return f(CurveTypes<FrBls, FqBls>{});
+    case B2M_CURVE_BN254: return f(CurveTypes<FrBn, FqBn>{});
+    case B2M_CURVE_BLS12_377: return f(CurveTypes<FrBls377, FqBls377>{});
+  }
+  throw Error(B2M_ERR_INVALID_ARG, "unknown curve id");
+}
+// B2M_ERR_INVALID_ARG unless curve is a known curve id
+inline void require_curve(int curve) {
+  with_curve(curve, [](auto) {});
+}
+}  // namespace b2m
 
 struct b2m_srs {
   b2m_ctx* ctx;
@@ -53,6 +87,7 @@ struct b2m_srs {
   size_t n_g, n_gamma;
   std::unique_ptr<b2m::Msm<b2m::FrBls, b2m::FqBls>> bls;
   std::unique_ptr<b2m::Msm<b2m::FrBn, b2m::FqBn>> bn;
+  std::unique_ptr<b2m::Msm<b2m::FrBls377, b2m::FqBls377>> bls377;
   // gamma_idx[k] = the power of beta held in slot k of the powers_of_gamma_g (they live in the window
   // tables right after the G1 powers: see Msm::n_extra)
   std::vector<uint64_t> gamma_idx;
@@ -68,20 +103,26 @@ struct b2m_srs {
   b2m::MsmLayout layout;    // the planned layout and the model's figures for it
   size_t budget = 0;        // pool bytes available when the key was created
 
+  // the key's MSM (std::unique_ptr) of the curve whose scalar field is Fr
+  template <class Fr>
+  auto& msm() {
+    if constexpr (std::is_same<Fr, b2m::FrBls>::value) return bls;
+    else if constexpr (std::is_same<Fr, b2m::FrBn>::value) return bn;
+    else return bls377;
+  }
+
   b2m_srs(b2m_ctx* c, int curve_, const uint64_t* g, size_t ng, const uint64_t* gamma, const uint64_t* gidx, size_t ngamma,
           int window_bits, int window_tables)
       : ctx(c), curve(curve_), n_g(ng), n_gamma(ngamma) {
     using namespace b2m;
     for (size_t k = 0; k < ngamma; k++) gamma_idx.push_back(gidx ? gidx[k] : k);
-    if (curve == B2M_CURVE_BLS12_381) {
-      plan<FrBls, FqBls>(window_bits, window_tables);
-      bls.reset(new Msm<FrBls, FqBls>(c->cx, reinterpret_cast<const Affine<FqBls>*>(g), ng, reinterpret_cast<const Affine<FqBls>*>(gamma), ngamma,
+    with_curve(curve, [&](auto t) {
+      using Fr = typename decltype(t)::Fr;
+      using Fq = typename decltype(t)::Fq;
+      plan<Fr, Fq>(window_bits, window_tables);
+      msm<Fr>().reset(new Msm<Fr, Fq>(c->cx, reinterpret_cast<const Affine<Fq>*>(g), ng, reinterpret_cast<const Affine<Fq>*>(gamma), ngamma,
                                       layout.c, false, layout.T, layout.max_pairs));
-    } else {
-      plan<FrBn, FqBn>(window_bits, window_tables);
-      bn.reset(new Msm<FrBn, FqBn>(c->cx, reinterpret_cast<const Affine<FqBn>*>(g), ng, reinterpret_cast<const Affine<FqBn>*>(gamma), ngamma,
-                                  layout.c, false, layout.T, layout.max_pairs));
-    }
+    });
     c->cx.sync();
   }
 
@@ -180,10 +221,16 @@ struct b2m_srs {
     fclose(f);
     return kb == (size_t)-1 ? kb : kb * 1024;
   }
-  int window_bits() const { return bls ? bls->c : bn->c; }
-  int window_tables() const { return bls ? bls->T : bn->T; }
-  int affine_levels() const { return bls ? bls->affine_levels : bn->affine_levels; }
-  size_t affine_min_refs() const { return bls ? bls->affine_min_refs : bn->affine_min_refs; }
+  template <class G>
+  auto with_msm(G&& g) const {
+    if (bls) return g(*bls);
+    if (bn) return g(*bn);
+    return g(*bls377);
+  }
+  int window_bits() const { return with_msm([](const auto& m) { return m.c; }); }
+  int window_tables() const { return with_msm([](const auto& m) { return m.T; }); }
+  int affine_levels() const { return with_msm([](const auto& m) { return m.affine_levels; }); }
+  size_t affine_min_refs() const { return with_msm([](const auto& m) { return m.affine_min_refs; }); }
 };
 
 

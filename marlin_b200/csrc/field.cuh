@@ -383,5 +383,7 @@ using FrBls = Fp<BlsFrParams>;
 using FqBls = Fp<BlsFqParams>;
 using FrBn = Fp<BnFrParams>;
 using FqBn = Fp<BnFqParams>;
+using FrBls377 = Fp<Bls377FrParams>;
+using FqBls377 = Fp<Bls377FqParams>;
 
 }  // namespace b2m

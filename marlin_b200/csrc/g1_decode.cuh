@@ -4,13 +4,15 @@
 // ark-serialize 0.3 `CanonicalDeserialize` of a short-Weierstrass affine point in compressed form [U ark-ec
 // short_weierstrass_jacobian.rs, ark-serialize SWFlags]: x little-endian in sizeof(Fq) bytes, the two top bits of the last
 // byte are flags (bit 7: y is the larger of the two roots, bit 6: the point at infinity; both set is not a flag value).
-// y = (x^3 + b)^((p + 1) / 4) (both base fields are 3 mod 4), checked by squaring.  The uncompressed form is x || y with the
+// y = sqrt(x^3 + b) (fq_sqrt: one exponentiation for BLS12-381 and BN254, Tonelli-Shanks for BLS12-377).  The uncompressed form is x || y with the
 // flags in y's last byte; `deserialize_uncompressed` checks x, y < p, and both forms check the curve equation and the
 // prime-order subgroup [U].  BN254 G1 has cofactor 1: every curve point passes.  BLS12-381 G1 has a cofactor; its subgroup
 // test is the endomorphism one of Scott, "A note on group membership tests for G1, G2 and GT on BLS pairing-friendly curves"
 // (2021): with phi(x, y) = (omega x, y), omega a cube root of unity in Fq, P is in G1 iff phi(P) = -u^2 P, u = -0xd201000000010000
 // the curve parameter.  That is two multiplications by the 64-bit |u| (126 doublings, 10 additions) instead of r * P
-// (255 doublings, ~128 additions); g1_times_r_is_inf keeps the definitional test for the tests.
+// (255 doublings, ~128 additions); g1_times_r_is_inf keeps the definitional test for the tests.  BLS12-377 G1 uses the same test
+// with its own u = 0x8508c00000000001 and omega (u^2 does not depend on the sign of u).  Its b = 1, so x = 0 decompresses to
+// (0, +-1), a point of order 3 that the subgroup test rejects.
 #pragma once
 #include "curve.cuh"
 #include "field.cuh"
@@ -52,6 +54,20 @@ struct G1Curve<FqBls> {
     const uint32_t w[12] = {0x798a64e8u, 0x30f1361bu, 0x7ece5a2au, 0xf3b8ddabu, 0xc61577f7u, 0x16a8ca3au,
                             0x74fd029bu, 0xc26a2ff8u, 0x60701c6eu, 0x3636b766u, 0x241b6160u, 0x051ba4abu};
     FqBls c;
+    for (int i = 0; i < 12; i++) c.l[i] = w[i];
+    return c;
+  }
+};
+template <>
+struct G1Curve<FqBls377> {
+  static constexpr uint32_t b = 1;
+  static constexpr bool has_cofactor = true;
+  using Fr = FrBls377;
+  static constexpr uint64_t u_abs = 0x8508c00000000001ull;
+  B2M_HD static FqBls377 omega() {  // 2^((q - 1) / 3), the cube root of unity with phi(g) = -u^2 g (Montgomery form)
+    const uint32_t w[12] = {0x5a7b8727u, 0x2c766f92u, 0x253d58b5u, 0x03d7f6b0u, 0xec122131u, 0x838ec0deu,
+                            0xf658bb10u, 0xbd5eb3e9u, 0x6ed3e52eu, 0x6942bd12u, 0xdd04ed6au, 0x01673786u};
+    FqBls377 c;
     for (int i = 0; i < 12; i++) c.l[i] = w[i];
     return c;
   }

@@ -1,8 +1,9 @@
 // G2 arithmetic over Fq2, host/device shared: the SRS loader decodes and subgroup-checks G2 points on the GPU (ark_points.cuh),
 // the host builds the G2 half of `KZG10::setup` with the same code (g2_host.hpp), and tests/ compile it for the host.
 //
-// Fq2 = Fq[u] / (u^2 + 1) for both supported curves; E'(Fq2): y^2 = x^3 + b' with b' = 4 (1 + u) (BLS12-381, M-type twist)
-// and b' = 3 / (9 + u) (BN254, D-type twist).  The group-law formulas below never need b'.
+// Fq2 = Fq[u] / (u^2 + beta): beta = 1 for BLS12-381 and BN254, 5 for BLS12-377.  E'(Fq2): y^2 = x^3 + b' with
+// b' = 4 (1 + u) (BLS12-381, M-type twist), b' = 3 / (9 + u) (BN254, D-type twist) and b' = 1 / u (BLS12-377, D-type twist).
+// The group-law formulas below never need b'.
 #pragma once
 #include <cstdint>
 
@@ -10,9 +11,25 @@
 
 namespace b2m {
 
+// beta of Fq2 = Fq[u] / (u^2 + beta)
+template <class Fq>
+struct Fq2Beta {
+  static constexpr uint32_t value = 1;
+};
+template <>
+struct Fq2Beta<FqBls377> {
+  static constexpr uint32_t value = 5;
+};
+
 template <class Fq>
 struct Fq2 {
+  static constexpr uint32_t beta = Fq2Beta<Fq>::value;
+  static_assert(beta == 1 || beta == 5, "Fq2: u^2 = -1 or -5");
   Fq c0, c1;
+  B2M_HD static Fq mul_beta(const Fq& a) {
+    if constexpr (beta == 1) return a;
+    else return a.dbl().dbl() + a;
+  }
   B2M_HD static Fq2 zero() { return Fq2{Fq::zero(), Fq::zero()}; }
   B2M_HD static Fq2 one() { return Fq2{Fq::one(), Fq::zero()}; }
   B2M_HD bool is_zero() const { return c0.is_zero() && c1.is_zero(); }
@@ -20,15 +37,15 @@ struct Fq2 {
   B2M_HD bool operator!=(const Fq2& o) const { return !(*this == o); }
   B2M_HD friend Fq2 operator+(const Fq2& a, const Fq2& b) { return Fq2{a.c0 + b.c0, a.c1 + b.c1}; }
   B2M_HD friend Fq2 operator-(const Fq2& a, const Fq2& b) { return Fq2{a.c0 - b.c0, a.c1 - b.c1}; }
-  B2M_HD friend Fq2 operator*(const Fq2& a, const Fq2& b) {  // Karatsuba, u^2 = -1
+  B2M_HD friend Fq2 operator*(const Fq2& a, const Fq2& b) {  // Karatsuba, u^2 = -beta
     const Fq v0 = a.c0 * b.c0, v1 = a.c1 * b.c1;
-    return Fq2{v0 - v1, (a.c0 + a.c1) * (b.c0 + b.c1) - v0 - v1};
+    return Fq2{v0 - mul_beta(v1), (a.c0 + a.c1) * (b.c0 + b.c1) - v0 - v1};
   }
   B2M_HD Fq2 sqr() const { return (*this) * (*this); }
   B2M_HD Fq2 dbl() const { return Fq2{c0.dbl(), c1.dbl()}; }
   B2M_HD Fq2 neg() const { return Fq2{c0.neg(), c1.neg()}; }
-  B2M_HD Fq2 inverse() const {  // (c0 - c1 u) / (c0^2 + c1^2)
-    const Fq n = (c0.sqr() + c1.sqr()).inverse();
+  B2M_HD Fq2 inverse() const {  // (c0 - c1 u) / (c0^2 + beta c1^2)
+    const Fq n = (c0.sqr() + mul_beta(c1.sqr())).inverse();
     return Fq2{c0 * n, (c1 * n).neg()};
   }
 };
@@ -134,6 +151,16 @@ struct G2Curve<FqBn> {
     return r;
   }
 };
+template <>
+struct G2Curve<FqBls377> {
+  B2M_HD static Fq2<FqBls377> b() {  // 1 / u = -u / 5
+    const uint32_t c1[12] = {0x66666685u, 0x80722666u, 0x899999a9u, 0x8df55926u, 0xd64f34cfu, 0x7fe4561au,
+                             0xb6e4f01bu, 0xb95da6d8u, 0xfc142743u, 0x4b747cccu, 0x70f49f43u, 0x0039c3fau};
+    Fq2<FqBls377> r{FqBls377::zero(), FqBls377::zero()};
+    for (int i = 0; i < 12; i++) r.c1.l[i] = c1[i];
+    return r;
+  }
+};
 
 // a / 2 (the Montgomery form halves like the value: p is odd and below 2^(32N - 1), so a + p never carries out)
 template <class Fq>
@@ -149,21 +176,58 @@ B2M_HD Fq fq_halve(const Fq& a) {
   return t;
 }
 
-// a^((p + 1) / 4), a square root of a when one exists (both base fields are 3 mod 4); true iff it squares back to a
+// A square root of a when one exists; true iff a is a square.  p = 3 mod 4 (TWO_ADICITY 1: BLS12-381, BN254): a^((p + 1) / 4),
+// checked by squaring.  Otherwise (BLS12-377: p - 1 = 2^46 t) Tonelli-Shanks with the 2^s-th root of unity g^t of the field's
+// non-residue generator g: x = a^((t + 1) / 2), b = a^t; while b != 1, find the least k with b^(2^k) = 1 (k = m means a is not
+// a square), then x *= c^(2^(m - k - 1)), c = that squared, b *= c, m = k.  One exponentiation plus at most s (s + 1) / 2 squarings.
 template <class Fq>
 B2M_HD bool fq_sqrt(const Fq& a, Fq* out) {
   constexpr int N = Fq::N;
-  uint32_t e[N];  // (p + 1) / 4: p = 3 mod 4, so p + 1 carries out of limb 0 only when it is 0xffffffff (never here)
-  for (int i = 0; i < N; i++) e[i] = Fq::Params::mod(i);
-  e[0] += 1u;
-  for (int i = 0; i < N - 1; i++) e[i] = (e[i] >> 2) | (e[i + 1] << 30);
-  e[N - 1] >>= 2;
-  *out = a.pow_limbs(e, N);
-  return out->sqr() == a;
+  if constexpr (Fq::Params::TWO_ADICITY == 1) {
+    uint32_t e[N];  // (p + 1) / 4: p = 3 mod 4, so p + 1 carries out of limb 0 only when it is 0xffffffff (never here)
+    for (int i = 0; i < N; i++) e[i] = Fq::Params::mod(i);
+    e[0] += 1u;
+    for (int i = 0; i < N - 1; i++) e[i] = (e[i] >> 2) | (e[i + 1] << 30);
+    e[N - 1] >>= 2;
+    *out = a.pow_limbs(e, N);
+    return out->sqr() == a;
+  } else {
+    if (a.is_zero()) {
+      *out = a;
+      return true;
+    }
+    uint32_t e[N];
+    for (int i = 0; i < N; i++) e[i] = Fq::Params::odd_half(i);
+    const Fq w = a.pow_limbs(e, N);  // a^((t - 1) / 2)
+    Fq x = a * w, b = x * w, c;
+    for (int i = 0; i < N; i++) c.l[i] = Fq::Params::root(i);
+    const Fq one = Fq::one();
+    int m = Fq::Params::TWO_ADICITY;
+    while (b != one) {
+      int k = 0;
+      for (Fq b2 = b; b2 != one; b2 = b2.sqr())
+        if (++k == m) return false;
+      for (int j = 0; j < m - k - 1; j++) c = c.sqr();
+      x = x * c;
+      c = c.sqr();
+      b = b * c;
+      m = k;
+    }
+    *out = x;
+    return true;
+  }
 }
 
-// Square root in Fq2 for p = 3 mod 4 by the norm ("complex") method: with n = sqrt(c0^2 + c1^2) in Fq, x = sqrt((c0 +- n) / 2)
-// and y = c1 / (2 x) give (x + y u)^2 = c0 + c1 u.  Three Fq exponentiations and one inversion.  False if a is not a square.
+// a / beta (beta = 1: a itself)
+template <class Fq>
+B2M_HD Fq fq2_div_beta(const Fq& a) {
+  if constexpr (Fq2<Fq>::beta == 1) return a;
+  else return a * Fq::from_u64(Fq2<Fq>::beta).inverse();
+}
+
+// Square root in Fq2 by the norm ("complex") method: with n = sqrt(c0^2 + beta c1^2) in Fq, x = sqrt((c0 +- n) / 2) and
+// y = c1 / (2 x) give (x + y u)^2 = x^2 - beta y^2 + 2 x y u = c0 + c1 u.  Three Fq square roots and one inversion.  False if
+// a is not a square.
 template <class Fq>
 B2M_HD bool fq2_sqrt(const Fq2<Fq>& a, Fq2<Fq>* out) {
   Fq s;
@@ -172,14 +236,14 @@ B2M_HD bool fq2_sqrt(const Fq2<Fq>& a, Fq2<Fq>* out) {
       *out = Fq2<Fq>{s, Fq::zero()};
       return true;
     }
-    if (fq_sqrt(a.c0.neg(), &s)) {  // (s u)^2 = -s^2
+    if (fq_sqrt(fq2_div_beta<Fq>(a.c0.neg()), &s)) {  // (s u)^2 = -beta s^2
       *out = Fq2<Fq>{Fq::zero(), s};
       return true;
     }
     return false;
   }
   Fq n;
-  if (!fq_sqrt(a.c0.sqr() + a.c1.sqr(), &n)) return false;
+  if (!fq_sqrt(a.c0.sqr() + Fq2<Fq>::mul_beta(a.c1.sqr()), &n)) return false;
   Fq x;
   if (!fq_sqrt(fq_halve(a.c0 + n), &x) && !fq_sqrt(fq_halve(a.c0 - n), &x)) return false;
   *out = Fq2<Fq>{x, a.c1 * x.dbl().inverse_fast()};

@@ -6,10 +6,10 @@
 //
 // Only "product == 1" is ever asked, so any non-degenerate bilinear pairing serves.  This is the reduced Tate pairing
 // over the single extension
-//     Fq12 = Fq[w] / (w^12 - 2 alpha w^6 + alpha^2 + 1)     (w^6 = xi = alpha + u, u^2 = -1)
-// with alpha = 1 (BLS12-381) or 9 (BN254).  G2 points (on the twist over Fq2) are mapped into E(Fq12) by the untwisting
-// isomorphism: M-type (BLS12-381, y^2 = x^3 + b xi): (x, y) -> (x / w^2, y / w^3); D-type (BN254, y^2 = x^3 + b / xi):
-// (x, y) -> (x w^2, y w^3).  The Miller loop runs over the bits of r with lines through multiples of the G1 argument
+//     Fq12 = Fq[w] / (w^12 - 2 alpha w^6 + alpha^2 + beta)     (w^6 = xi = alpha + u, u^2 = -beta)
+// with (alpha, beta) = (1, 1) (BLS12-381), (9, 1) (BN254) or (0, 5) (BLS12-377).  G2 points (on the twist over Fq2) are mapped
+// into E(Fq12) by the untwisting isomorphism: M-type (BLS12-381, y^2 = x^3 + b xi): (x, y) -> (x / w^2, y / w^3); D-type
+// (BN254, BLS12-377, y^2 = x^3 + b / xi): (x, y) -> (x w^2, y w^3).  The Miller loop runs over the bits of r with lines through multiples of the G1 argument
 // (slopes in Fq, vertical lines dropped: they die in the final exponentiation), all pairs sharing one accumulator;
 // the final exponentiation is (p^6 - 1)(p^2 + 1) through the Frobenius map, then the hard part (p^4 - p^2 + 1) / r by
 // square-and-multiply.
@@ -30,7 +30,7 @@ struct PairingParams;
 template <>
 struct PairingParams<FqBls> {
   using Fr = FrBls;
-  static constexpr uint64_t alpha = 1, b = 4;
+  static constexpr uint64_t alpha = 1, beta = 1, b = 4;
   static constexpr bool m_twist = true;
   // (p^4 - p^2 + 1) / r
   static const char* hard_exp() {
@@ -42,11 +42,22 @@ struct PairingParams<FqBls> {
 template <>
 struct PairingParams<FqBn> {
   using Fr = FrBn;
-  static constexpr uint64_t alpha = 9, b = 3;
+  static constexpr uint64_t alpha = 9, beta = 1, b = 3;
   static constexpr bool m_twist = false;
   static const char* hard_exp() {
     return "1baaa710b0759ad331ec15183177faf6c0eb522d5b122784e529a5861876f6b3b1b1355d189227d79581e16f3fd90c66b887d56d5095f23aaa441e3954bcf8adcc7b44c"
            "87cdbacff1154e7e1da014fd5abf5cc4f49c36d4e81bb482ccdf42b1";
+  }
+};
+template <>
+struct PairingParams<FqBls377> {
+  using Fr = FrBls377;
+  static constexpr uint64_t alpha = 0, beta = 5, b = 1;
+  static constexpr bool m_twist = false;
+  static const char* hard_exp() {
+    return "6d616e43720774d7d810d5cbdf0576728e56efc3bf3b4074a5448da5cfbef98d9c2cce3b25c548afd84225b34ccc65eca9c9678a845497a9781d8129911a8d889"
+           "828282015fcd1c3fa1470f8b2d1eefd89535f9b5aaae0551dffcf72fb0bd948d5f4548283abcaf63f0a34fcb827dc8f4db069bf65f4f6974b4ff0fa27719b834b"
+           "6904468768c0eaeea22e68002e16ba88600000000000000000000001";
   }
 };
 
@@ -112,6 +123,7 @@ struct Fq12 {
     return r;
   }
   // schoolbook product, zero coefficients skipped (the Miller loop's lines have five), reduced with w^12 = c6 w^6 - c0
+  // (c6 = 2 alpha, c0 = alpha^2 + beta)
   friend Fq12 operator*(const Fq12& a, const Fq12& b) {
     Fq t[23];
     for (auto& x : t) x = Fq::zero();
@@ -122,7 +134,7 @@ struct Fq12 {
       if (a.c[i].is_zero()) continue;
       for (int k = 0; k < nb; k++) t[i + nzb[k]] = t[i + nzb[k]] + a.c[i] * b.c[nzb[k]];
     }
-    const Fq c6 = Fq::from_u64(2 * PairingParams<Fq>::alpha), c0 = Fq::from_u64(PairingParams<Fq>::alpha * PairingParams<Fq>::alpha + 1);
+    const Fq c6 = Fq::from_u64(2 * PairingParams<Fq>::alpha), c0 = Fq::from_u64(PairingParams<Fq>::alpha * PairingParams<Fq>::alpha + PairingParams<Fq>::beta);
     for (int k = 22; k >= 12; k--) {
       if (t[k].is_zero()) continue;
       t[k - 6] = t[k - 6] + c6 * t[k];
@@ -163,7 +175,7 @@ struct PairingTables {
     w.c[1] = Fq::one();
     E w2 = w * w, w3 = w2 * w;
     if (PairingParams<Fq>::m_twist) {  // w^-1 = (c6 w^5 - w^11) / c0
-      const Fq c0 = Fq::from_u64(PairingParams<Fq>::alpha * PairingParams<Fq>::alpha + 1);
+      const Fq c0 = Fq::from_u64(PairingParams<Fq>::alpha * PairingParams<Fq>::alpha + PairingParams<Fq>::beta);
       E wi = E::zero();
       wi.c[5] = Fq::from_u64(2 * PairingParams<Fq>::alpha);
       wi.c[11] = Fq::one().neg();

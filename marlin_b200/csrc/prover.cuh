@@ -31,6 +31,8 @@ IndexBase* make_index_bls(b2m_srs* srs, int pc, size_t num_constraints, size_t n
                           const b2m_matrix* a, const b2m_matrix* b, const b2m_matrix* c);
 IndexBase* make_index_bn(b2m_srs* srs, int pc, size_t num_constraints, size_t num_variables, size_t num_instance,
                          const b2m_matrix* a, const b2m_matrix* b, const b2m_matrix* c);
+IndexBase* make_index_bls377(b2m_srs* srs, int pc, size_t num_constraints, size_t num_variables, size_t num_instance,
+                             const b2m_matrix* a, const b2m_matrix* b, const b2m_matrix* c);
 
 // An index from a key file (b2m_index_load).  bad receives (vector, index, reason) of the first failed check.
 IndexBase* load_index_bls(b2m_srs* srs, int pc, size_t num_constraints, size_t num_variables, size_t num_instance, size_t num_non_zero,
@@ -39,6 +41,9 @@ IndexBase* load_index_bls(b2m_srs* srs, int pc, size_t num_constraints, size_t n
 IndexBase* load_index_bn(b2m_srs* srs, int pc, size_t num_constraints, size_t num_variables, size_t num_instance, size_t num_non_zero,
                          const b2m_matrix* a, const b2m_matrix* b, const b2m_matrix* c, const uint8_t* const* vectors, const size_t* lens,
                          const uint64_t* comms_xy, bool check_commitments, size_t bad[3]);
+IndexBase* load_index_bls377(b2m_srs* srs, int pc, size_t num_constraints, size_t num_variables, size_t num_instance, size_t num_non_zero,
+                             const b2m_matrix* a, const b2m_matrix* b, const b2m_matrix* c, const uint8_t* const* vectors, const size_t* lens,
+                             const uint64_t* comms_xy, bool check_commitments, size_t bad[3]);
 
 // `PC::commit` over host polynomials (Level 1 of include/b2m.h)
 void pc_commit_bls(b2m_srs* srs, int pc, size_t n_polys, const uint64_t* const* coeffs, const size_t* n_coeffs,
@@ -47,6 +52,9 @@ void pc_commit_bls(b2m_srs* srs, int pc, size_t n_polys, const uint64_t* const* 
 void pc_commit_bn(b2m_srs* srs, int pc, size_t n_polys, const uint64_t* const* coeffs, const size_t* n_coeffs,
                   const int64_t* degree_bounds, const int64_t* hiding_bounds, b2m_rng* rng, uint64_t* out_comm_xy,
                   uint64_t* out_shifted_xy, uint64_t* out_rand, uint64_t* out_shifted_rand, size_t rand_stride);
+void pc_commit_bls377(b2m_srs* srs, int pc, size_t n_polys, const uint64_t* const* coeffs, const size_t* n_coeffs,
+                      const int64_t* degree_bounds, const int64_t* hiding_bounds, b2m_rng* rng, uint64_t* out_comm_xy,
+                      uint64_t* out_shifted_xy, uint64_t* out_rand, uint64_t* out_shifted_rand, size_t rand_stride);
 
 // `PC::open_combinations` over host polynomials, and `PC::open` as its one-point case (Level 1 of include/b2m.h)
 void pc_open_combinations_bls(b2m_srs* srs, int pc, int64_t max_degree_bound, size_t n_polys, const uint64_t* const* coeffs, const size_t* n_coeffs,
@@ -59,5 +67,11 @@ void pc_open_combinations_bn(b2m_srs* srs, int pc, int64_t max_degree_bound, siz
                              size_t n_lcs, const size_t* lc_term_off, const int64_t* lc_poly, const uint64_t* lc_coeff, size_t n_queries,
                              const size_t* query_lc, const size_t* query_point, size_t n_points, const uint64_t* points,
                              const uint64_t* opening_challenge, uint64_t* out_w_xy, int* out_has_random_v, uint64_t* out_random_v);
+void pc_open_combinations_bls377(b2m_srs* srs, int pc, int64_t max_degree_bound, size_t n_polys, const uint64_t* const* coeffs,
+                                 const size_t* n_coeffs, const int64_t* degree_bounds, const int* hiding, const uint64_t* rands,
+                                 const uint64_t* shifted_rands, size_t rand_stride, size_t n_lcs, const size_t* lc_term_off, const int64_t* lc_poly,
+                                 const uint64_t* lc_coeff, size_t n_queries, const size_t* query_lc, const size_t* query_point, size_t n_points,
+                                 const uint64_t* points, const uint64_t* opening_challenge, uint64_t* out_w_xy, int* out_has_random_v,
+                                 uint64_t* out_random_v);
 
 }  // namespace b2m

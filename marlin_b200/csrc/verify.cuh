@@ -30,5 +30,6 @@ struct VkArgs {
 
 VerifierBase* make_verifier_bls(Ctx& cx, const VkArgs& a);
 VerifierBase* make_verifier_bn(Ctx& cx, const VkArgs& a);
+VerifierBase* make_verifier_bls377(Ctx& cx, const VkArgs& a);
 
 }  // namespace b2m

@@ -108,7 +108,7 @@ def run(args, tables, cap):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--log-n", type=int, default=20)
-    ap.add_argument("--curve", default="bls12_381", choices=["bls12_381", "bn254"])
+    ap.add_argument("--curve", default="bls12_381", choices=["bls12_381", "bn254", "bls12_377"])
     ap.add_argument("--pc", default="marlin_kzg10", choices=["marlin_kzg10", "sonic_kzg10"])
     ap.add_argument("--limit-gb", type=float, default=0.0, help="device-memory limit of the context (0: free device memory)")
     ap.add_argument("--tables", type=int, nargs="*", default=[0], help="forced window tables, one run each (0: the planned layout)")

@@ -5,7 +5,7 @@ H2D, G1 decode, G2 decode, D2H (the library's CUDA-event spans) and the window-t
 limit, one JSON line per file.  SonicKZG10's G2 half is stood in for by 2^k neg_powers_of_h repeating a few valid points
 (decode cost does not depend on the value).
 
-    python tools/bench_srs_load.py [--log-powers 20 22] [--curves bls12_381 bn254]
+    python tools/bench_srs_load.py [--log-powers 20 22] [--curves bls12_381 bn254 bls12_377]
 """
 import argparse
 import json
@@ -26,7 +26,7 @@ from marlin_b200 import api, srsfile  # noqa: E402
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--log-powers", type=int, nargs="+", default=[20, 22])
-    ap.add_argument("--curves", nargs="+", default=["bls12_381", "bn254"])
+    ap.add_argument("--curves", nargs="+", default=["bls12_381", "bn254"], choices=["bls12_381", "bn254", "bls12_377"])
     args = ap.parse_args()
     card = gpu_card()
     with tempfile.TemporaryDirectory() as tmp:

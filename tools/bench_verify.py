@@ -35,7 +35,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=4096, help="proofs per verify_batch call")
     ap.add_argument("--log-n", type=int, default=10, help="log2 of the constraints of the verified circuit")
-    ap.add_argument("--curve", default="bls12_381", choices=["bls12_381", "bn254"])
+    ap.add_argument("--curve", default="bls12_381", choices=["bls12_381", "bn254", "bls12_377"])
     ap.add_argument("--pc", default="marlin_kzg10", choices=["marlin_kzg10", "sonic_kzg10"])
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=1)
