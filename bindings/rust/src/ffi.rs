@@ -92,6 +92,8 @@ extern "C" {
                        out_has_random_v: *mut c_int, out_random_v: *mut u64) -> c_int;
     pub fn b2m_g1_powers(ctx: *mut b2m_ctx, curve: c_int, g_xy: *const u64, beta: *const u64, n: usize, out_powers_xy: *mut u64) -> c_int;
     pub fn b2m_fixed_base_msm(ctx: *mut b2m_ctx, curve: c_int, g_xy: *const u64, scalars: *const u64, n: usize, out_xy: *mut u64) -> c_int;
+    pub fn b2m_pairing_check(ctx: *mut b2m_ctx, curve: c_int, n_g2: usize, g2: *const u8, n_products: usize, product_off: *const usize,
+                             g1_xy: *const u64, g2_index: *const u32, verdicts: *mut c_int) -> c_int;
     pub fn b2m_trim(srs: *mut b2m_srs, pc_variant: c_int, supported_degree: usize, supported_hiding_bound: usize,
                     enforced_degree_bounds: *const u64, n_bounds: usize, out: *mut *mut b2m_ck) -> c_int;
     pub fn b2m_ck_destroy(ck: *mut b2m_ck);

@@ -180,6 +180,18 @@ int b2m_g1_decode_ark(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, i
                       size_t* bad_index, int* bad_reason);
 int b2m_g2_decode_ark(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, int compressed, uint8_t* out_uncompressed,
                       size_t* bad_index, int* bad_reason);
+/* `PairingEngine::product_of_pairings(pairs).is_one()` [U ark-ec 0.3] for many products at once.  g2: n_g2 distinct G2 points
+ * as uncompressed ark-serialize bytes (the b2m_g2_scalar_muls / b2m_vk_create form).  Product k is the pairs
+ * [product_off[k], product_off[k+1]): G1 point g1_xy[j] (affine Montgomery, (0,0) = infinity) with G2 point g2_index[j].
+ * verdicts[k] = 1 iff the product is one (an empty product is one).  A pair with either point at infinity contributes 1.
+ * Runs on the GPU, one thread per product, with the optimal-ate Miller loop and final exponentiation of pairing.cuh; the G2
+ * line coefficients are computed once per call on the host.  Products go to the GPU in chunks of at most 2^16 products and
+ * max(2^18, pairs of the largest product) pairs, so device scratch stays bounded by that whatever n_products is.
+ * Input checks: a G2 point that is non-canonical or off the twist fails with B2M_ERR_SERIALIZATION, a G1 point off the curve
+ * (or with limbs not below p) with B2M_ERR_INVALID_ARG, as do decreasing offsets and g2_index[j] >= n_g2; b2m_last_error()
+ * names the index.  Subgroup membership is the caller's job: b2m_g1_decode_ark / b2m_g2_decode_ark check it. */
+int b2m_pairing_check(b2m_ctx* ctx, int curve, size_t n_g2, const uint8_t* g2, size_t n_products, const size_t* product_off,
+                      const uint64_t* g1_xy, const uint32_t* g2_index, int* verdicts);
 /* `CanonicalSerialize::serialize` (compressed) of G1 points given as affine Montgomery limbs (GPU), and of G2 points given as
  * uncompressed canonical bytes (host: no square root is needed).  Infinity is written as zero coordinates + bit 6. */
 int b2m_g1_to_compressed(b2m_ctx* ctx, int curve, const uint64_t* points_xy, size_t n, uint8_t* out);
@@ -393,8 +405,8 @@ void b2m_vk_destroy(b2m_vk* vk);
  * verdicts[i] = 1 accepted, 0 rejected by the check, -1 malformed bytes (framing, trailing bytes, x >= p, a point not on the
  * curve or outside the prime-order subgroup, an evaluation or random_v >= r).  Malformed proofs are verdicts, not errors.
  * The proofs' G1 points are decoded on the GPU; all checks of the batch are folded with one 128-bit randomiser per (proof,
- * opening point) drawn from rng (which must be unpredictable to the prover) into a few MSMs on the GPU and one pairing
- * product on the host; a failing batch is bisected with fresh randomisers until every bad proof is isolated.
+ * opening point) drawn from rng (which must be unpredictable to the prover) into a few MSMs and one pairing product
+ * (b2m_pairing_check's kernel), all on the GPU; a failing batch is bisected with fresh randomisers until every bad proof is isolated.
  * rng == NULL fails with B2M_ERR_MISSING_RNG. */
 int b2m_verify_batch(b2m_vk* vk, size_t n, const uint64_t* const* public_inputs, const size_t* n_inputs,
                      const uint8_t* const* proofs, const size_t* proof_lens, b2m_rng* rng, int* verdicts);

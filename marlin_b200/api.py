@@ -411,6 +411,29 @@ def srs_gamma_powers(srs, idx):
     return np.stack(out)
 
 
+def pairing_check(ctx, curve, g2_points, products):
+    """`product_of_pairings(pairs).is_one()` for many products on the GPU (b2m_pairing_check).  curve: a C ABI curve id
+    (_lib.CURVE_*).  g2_points: a list of
+    uncompressed ark-serialize G2 byte strings; products: a list of products, each a list of (g1, k) pairs with g1 an array
+    of 2 * limbs uint64 (affine Montgomery, zeros = infinity) and k an index into g2_points.  Returns a list of bools."""
+    cid = curve
+    nq = _lib.LIMBS[cid][1]
+    off = np.zeros(len(products) + 1, dtype=np.uint64)
+    g1, idx = [], []
+    for k, pr in enumerate(products):
+        for pt, q in pr:
+            g1.append(np.asarray(pt, dtype=np.uint64).reshape(2 * nq))
+            idx.append(q)
+        off[k + 1] = len(idx)
+    g1a = np.concatenate(g1) if g1 else np.zeros(2 * nq, dtype=np.uint64)
+    idxa = np.asarray(idx or [0], dtype=np.uint32)
+    g2a = np.frombuffer(b"".join(g2_points) or b"\0", dtype=np.uint8)
+    out = np.zeros(max(1, len(products)), dtype=np.int32)
+    _lib.check(_lib.lib().b2m_pairing_check(ctx.handle, cid, len(g2_points), _lib.ptr(g2a), len(products), _lib.ptr(off), _lib.ptr(g1a),
+                                            _lib.ptr(idxa), _lib.ptr(out)))
+    return [bool(v) for v in out[:len(products)]]
+
+
 def domain_bytes(cid, size):
     """`Radix2EvaluationDomain::new(size)` as ark-serialize writes it (b2m_domain_ark)"""
     out = np.zeros(172, dtype=np.uint8)

@@ -280,6 +280,16 @@ int b2m_g2_decode_ark(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, i
       throw Error(B2M_ERR_SERIALIZATION, fmt("G2 point %zu: %s", bad.index, point_status_name(bad.reason)));
   });
 }
+int b2m_pairing_check(b2m_ctx* ctx, int curve, size_t n_g2, const uint8_t* g2, size_t n_products, const size_t* product_off,
+                      const uint64_t* g1_xy, const uint32_t* g2_index, int* verdicts) {
+  return guard([&] {
+    B2M_REQUIRE(ctx && (g2 || n_g2 == 0) && ((product_off && verdicts) || n_products == 0), B2M_ERR_INVALID_ARG, "null argument");
+    B2M_REQUIRE(n_products == 0 || product_off[n_products] == product_off[0] || (g1_xy && g2_index), B2M_ERR_INVALID_ARG, "null argument");
+    require_curve(curve);
+    ctx->cx.use();
+    with_curve(curve, [&](auto t) { pairing_check<typename decltype(t)::Fq>(ctx->cx, n_g2, g2, n_products, product_off, g1_xy, g2_index, verdicts); });
+  });
+}
 int b2m_g1_to_compressed(b2m_ctx* ctx, int curve, const uint64_t* points_xy, size_t n, uint8_t* out) {
   return guard([&] {
     B2M_REQUIRE(ctx && ((points_xy && out) || n == 0), B2M_ERR_INVALID_ARG, "null argument");

@@ -1,4 +1,5 @@
 #include "verify_impl.cuh"
 namespace b2m {
 VerifierBase* make_verifier_bls377(Ctx& cx, const VkArgs& a) { return new MarlinVerifier<FrBls377, FqBls377>(cx, a); }
+template void pairing_check<FqBls377>(Ctx&, size_t, const uint8_t*, size_t, const size_t*, const uint64_t*, const uint32_t*, int*);
 }  // namespace b2m

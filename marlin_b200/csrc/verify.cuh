@@ -28,6 +28,11 @@ struct VkArgs {
   const void* bound_points;
 };
 
+// b2m_pairing_check for one curve (pairing_impl.cuh; instantiated with the verifier of that curve)
+template <class Fq>
+void pairing_check(Ctx& cx, size_t n_g2, const uint8_t* g2, size_t n_products, const size_t* off, const uint64_t* g1_xy, const uint32_t* g2_index,
+                   int* verdicts);
+
 VerifierBase* make_verifier_bls(Ctx& cx, const VkArgs& a);
 VerifierBase* make_verifier_bn(Ctx& cx, const VkArgs& a);
 VerifierBase* make_verifier_bls377(Ctx& cx, const VkArgs& a);

@@ -7,20 +7,23 @@
 //                          bookkeeping of the PC scheme -> per proof and point a list of (Fr scalar, G1 base) terms of
 //                              e(plain + z W, h) * e(-W, beta h) * prod_d e(C_d, beta^-(D-d) h) = 1
 //   4. batch check         one 128-bit randomiser per (proof, point) from the caller's rng folds every equation into
-//                          MSM_A (plain + z W), MSM_B (W) and, for SonicKZG10, one MSM per bound -- all over the same
-//                          device-resident bases, shared bases (index commitments, g, gamma g, shift powers) once with
-//                          summed scalars -- and one host pairing product (pairing_host.hpp)
+//                          MSM_A (plain + z W), MSM_B (W) and, for SonicKZG10, one MSM per bound -- over the checked proofs'
+//                          slice of the device-resident bases plus the shared bases (index commitments, g, gamma g, shift
+//                          powers) with summed scalars -- and one pairing product, checked on the GPU (pairing_impl.cuh)
 //   5. bisection           a failing set is split in halves, each checked with fresh randomisers, until every bad proof is
-//                          isolated: m bad proofs cost O(m log N) extra checks
+//                          isolated: m bad proofs cost O(m log N) extra checks, made level by level (all checks of a level in
+//                          one MSM batch and one pairing launch), so O(log N) rounds
 #pragma once
 #include <algorithm>
 #include <chrono>
+#include <cstdint>
 #include <cstring>
 #include <thread>
 
 #include "capi_types.cuh"
 #include "g1_decode.cuh"
-#include "pairing_host.hpp"
+#include "pairing_host.hpp"  // g2_prepare: the on-twist check of the key's G2 points
+#include "pairing_impl.cuh"
 #include "prover_impl.cuh"  // MarlinIndex's ToBytes writers (the transcript encodes commitments as the prover does)
 #include "verify.cuh"
 
@@ -51,8 +54,7 @@ struct MarlinVerifier : VerifierBase {
   std::vector<Pt> shared;  // bases 0 .. shared.size()
   std::vector<uint64_t> bounds;
   size_t bidx_h, bidx_k;  // indices of |H| - 2 and |K| - 2 among the bounds
-  G2Prepared<Fq> h, beta_h;
-  std::vector<G2Prepared<Fq>> neg;  // SonicKZG10: beta^-(D - d) h per bound
+  std::unique_ptr<PairingG2Set<Fq>> g2set;  // h, beta_h, then SonicKZG10's beta^-(D - d) h per bound, prepared for the GPU pairing
   std::vector<uint8_t> vk_bytes;
 
   static size_t pow2_at_least(size_t n) {
@@ -82,6 +84,7 @@ struct MarlinVerifier : VerifierBase {
     }
     B2M_REQUIRE(bidx_h < a.n_bounds && bidx_k < a.n_bounds, B2M_ERR_INVALID_ARG, "the key must carry the degree bounds |H| - 2 = %zu and |K| - 2 = %zu",
                 H - 2, K - 2);
+    G2Prepared<Fq> h, beta_h;
     B2M_REQUIRE(g2_prepare<Fq>(a.h_bytes, &h) && g2_prepare<Fq>(a.beta_h_bytes, &beta_h), B2M_ERR_INVALID_ARG,
                 "h / beta_h is not a finite point of the G2 curve");
     for (size_t k = 0; k < a.n_bounds; k++) {
@@ -91,9 +94,13 @@ struct MarlinVerifier : VerifierBase {
         G2Prepared<Fq> q;
         B2M_REQUIRE(g2_prepare<Fq>(static_cast<const uint8_t*>(a.bound_points) + k * 4 * FQ_BYTES, &q), B2M_ERR_INVALID_ARG,
                     "neg_powers_of_h[%zu] is not a finite point of the G2 curve", k);
-        neg.push_back(q);
       }
     }
+    std::vector<uint8_t> g2b(a.h_bytes, a.h_bytes + 4 * FQ_BYTES);
+    g2b.insert(g2b.end(), a.beta_h_bytes, a.beta_h_bytes + 4 * FQ_BYTES);
+    if (pc == B2M_PC_SONIC_KZG10)
+      g2b.insert(g2b.end(), static_cast<const uint8_t*>(a.bound_points), static_cast<const uint8_t*>(a.bound_points) + a.n_bounds * 4 * FQ_BYTES);
+    g2set.reset(new PairingG2Set<Fq>(cx, g2b.size() / (4 * FQ_BYTES), g2b.data()));
     // IndexVerifierKey ToBytes [reference src/data_structures.rs:36-43]: index_info || index_comms
     put_u64(vk_bytes, nv);
     put_u64(vk_bytes, nc);
@@ -313,71 +320,111 @@ struct MarlinVerifier : VerifierBase {
     return true;
   }
 
-  // ---- 4. one randomised check over a set of proofs ------------------------------------------------------------------
+  // ---- 4. + 5. randomised checks, the bisection tree level by level ---------------------------------------------------
   struct Batch {
-    std::unique_ptr<Msm<Fr, Fq>> msm;
-    size_t n_bases = 0;
+    std::unique_ptr<Msm<Fr, Fq>> msm;  // bases: the proofs' points; extra bases: the shared ones
     std::vector<ProofEq> eqs;
+    std::vector<size_t> pt_lo, pt_hi;  // per equation: its proof's points [lo, hi) among the proof points
     double ms_msm = 0, ms_pairing = 0, ms_first = 0;
     int checks = 0;
   };
   using Clock = std::chrono::steady_clock;
   static double ms_since(Clock::time_point t) { return std::chrono::duration<double, std::milli>(Clock::now() - t).count(); }
 
-  bool check(Batch& B, const std::vector<size_t>& which, ZkSource<b2m_rng>& rng) const {
-    const Clock::time_point t_check = Clock::now();
-    const size_t nb = B.n_bases, nbound = bounds.size();
-    std::vector<Fr> sa(nb, Fr::zero()), sb(nb, Fr::zero());
-    std::vector<std::vector<Fr>> sd(pc == B2M_PC_SONIC_KZG10 ? nbound : 0);
-    std::vector<bool> used(nbound, false);
-    for (size_t i : which)
-      for (const PointEq& pe : B.eqs[i].pt) {
-        uint64_t lo = rng.next_u64(), hi = rng.next_u64();
-        const Fr r = fr_u128(lo, hi);
-        for (const Term& t : pe.plain) sa[t.base] = sa[t.base] + r * t.c;
-        sa[pe.w] = sa[pe.w] + r * pe.z;
-        sb[pe.w] = sb[pe.w] + r;
-        for (const auto& bt : pe.bounded) {
-          if (sd[bt.first].empty()) sd[bt.first].assign(nb, Fr::zero());
-          sd[bt.first][bt.second.base] = sd[bt.first][bt.second.base] + r * bt.second.c;
-          used[bt.first] = true;
+  // A node is a range [a, b) of equations (contiguous in proof order, so its proofs' points are one slice of the bases).
+  // The root is checked; a failing node of one proof is a bad proof, a failing larger node has both halves checked.  That is
+  // the depth-first bisection's set of checks, with the same randomisers per check (two 128-bit ones per proof), so the rng
+  // ends at the same position; they are only drawn level by level.  All checks of a level run their MSMs as one
+  // Msm::run_batch sequence (each MSM over its node's slice plus the shared bases) and their pairing products as one
+  // PairingG2Set::check launch.
+  void resolve(Batch& B, const std::vector<size_t>& proof_of, ZkSource<b2m_rng>& rng, int* verdicts) const {
+    const size_t S = shared.size();
+    std::vector<std::pair<size_t, size_t>> level{{0, B.eqs.size()}};
+    bool first = true;
+    while (!level.empty()) {
+      const Clock::time_point t_level = Clock::now();
+      // scalars: per MSM, its node's slice (len values) then the S shared bases
+      std::vector<Fr> sc;
+      std::vector<size_t> job_off, job_len, job_lo;
+      std::vector<std::vector<std::pair<size_t, uint32_t>>> node_jobs(level.size());  // (job, G2 point) per pair
+      for (size_t nd = 0; nd < level.size(); nd++) {
+        const size_t a = level[nd].first, b = level[nd].second, lo = B.pt_lo[a], len = B.pt_hi[b - 1] - lo;
+        auto new_job = [&](uint32_t g2) {
+          job_off.push_back(sc.size());
+          job_len.push_back(len);
+          job_lo.push_back(lo);
+          sc.resize(sc.size() + len + S, Fr::zero());
+          node_jobs[nd].push_back({job_off.size() - 1, g2});
+          return job_off.size() - 1;
+        };
+        const size_t ja = new_job(0), jb = new_job(1);  // plain + z W against h, W against beta h
+        std::vector<size_t> jd(bounds.size(), SIZE_MAX);
+        auto at = [&](size_t job, uint32_t base) -> Fr& { return base < S ? sc[job_off[job] + len + base] : sc[job_off[job] + (base - S - lo)]; };
+        for (size_t i = a; i < b; i++)
+          for (const PointEq& pe : B.eqs[i].pt) {
+            uint64_t rlo = rng.next_u64(), rhi = rng.next_u64();
+            const Fr r = fr_u128(rlo, rhi);
+            for (const Term& t : pe.plain) at(ja, t.base) = at(ja, t.base) + r * t.c;
+            at(ja, pe.w) = at(ja, pe.w) + r * pe.z;
+            at(jb, pe.w) = at(jb, pe.w) + r;
+            for (const auto& bt : pe.bounded) {
+              if (jd[bt.first] == SIZE_MAX) jd[bt.first] = new_job((uint32_t)(2 + bt.first));
+              at(jd[bt.first], bt.second.base) = at(jd[bt.first], bt.second.base) + r * bt.second.c;
+            }
+          }
+      }
+      Clock::time_point t0 = Clock::now();
+      for (Fr& x : sc) x = x.to_canonical();
+      const size_t nj = job_off.size();
+      DBuf<Fr> dsc(cx, sc.size());
+      DBuf<Pt> dres(cx, nj);
+      dsc.upload(sc.data(), sc.size());
+      for (size_t j0 = 0; j0 < nj; j0 += MSM_MAX_BATCH) {
+        MsmJob<Fr, Fq> jobs[MSM_MAX_BATCH];
+        const int m = (int)std::min<size_t>(MSM_MAX_BATCH, nj - j0);
+        for (int k = 0; k < m; k++) {
+          const size_t j = j0 + k;
+          jobs[k] = MsmJob<Fr, Fq>{dsc.p + job_off[j], false, job_len[j], job_lo[j], dsc.p + job_off[j] + job_len[j], S, 0, nullptr, 0, nullptr,
+                                   dres.p + j};
+        }
+        B.msm->run_batch(jobs, m);
+      }
+      std::vector<Pt> res(nj);
+      dres.download(res.data(), nj);
+      B.ms_msm += ms_since(t0);
+      t0 = Clock::now();
+      std::vector<Pt> g1;
+      std::vector<uint32_t> g2i;
+      std::vector<size_t> off{0};
+      for (size_t nd = 0; nd < level.size(); nd++) {
+        for (const auto& jq : node_jobs[nd]) {
+          const Pt& q = res[jq.first];
+          g1.push_back(jq.second == 1 ? Pt{q.x, q.y.neg()} : q);  // -W against beta h (infinity stays (0, 0))
+          g2i.push_back(jq.second);
+        }
+        off.push_back(g1.size());
+      }
+      std::vector<int> ok(level.size());
+      g2set->check(level.size(), off.data(), reinterpret_cast<const uint64_t*>(g1.data()), g2i.data(), ok.data());
+      B.ms_pairing += ms_since(t0);
+      B.checks += (int)level.size();
+      std::vector<std::pair<size_t, size_t>> next;
+      for (size_t nd = 0; nd < level.size(); nd++) {
+        const size_t a = level[nd].first, b = level[nd].second;
+        if (ok[nd] == 1) {
+          for (size_t i = a; i < b; i++) verdicts[proof_of[i]] = 1;
+        } else if (b - a == 1) {
+          verdicts[proof_of[a]] = 0;
+        } else {
+          const size_t half = (b - a) / 2;
+          next.push_back({a, a + half});
+          next.push_back({a + half, b});
         }
       }
-    Clock::time_point t0 = Clock::now();
-    auto msm = [&](std::vector<Fr>& s) {
-      for (Fr& x : s) x = x.to_canonical();
-      Pt out;
-      int inf = 0;
-      B.msm->run_host(0, reinterpret_cast<const uint64_t*>(s.data()), nb, reinterpret_cast<uint64_t*>(&out), &inf);
-      return out;
-    };
-    Pt A = msm(sa), Bw = msm(sb);
-    std::vector<std::pair<Pt, const G2Prepared<Fq>*>> pairs;
-    pairs.push_back({A, &h});
-    pairs.push_back({Pt{Bw.x, Bw.y.neg()}, &beta_h});  // (infinity stays (0, 0))
-    for (size_t k = 0; k < sd.size(); k++)
-      if (used[k]) pairs.push_back({msm(sd[k]), &neg[k]});
-    B.ms_msm += ms_since(t0);
-    t0 = Clock::now();
-    const bool ok = pairing_product_is_one(pairs);
-    B.ms_pairing += ms_since(t0);
-    if (B.checks++ == 0) B.ms_first = ms_since(t_check);
-    return ok;
-  }
-
-  void resolve(Batch& B, const std::vector<size_t>& which, const std::vector<size_t>& proof_of, ZkSource<b2m_rng>& rng, int* verdicts) const {
-    if (which.empty()) return;
-    if (check(B, which, rng)) {
-      for (size_t i : which) verdicts[proof_of[i]] = 1;
-      return;
+      if (first) B.ms_first = ms_since(t_level);
+      first = false;
+      level.swap(next);
     }
-    if (which.size() == 1) {
-      verdicts[proof_of[which[0]]] = 0;
-      return;
-    }
-    const size_t half = which.size() / 2;
-    resolve(B, std::vector<size_t>(which.begin(), which.begin() + half), proof_of, rng, verdicts);
-    resolve(B, std::vector<size_t>(which.begin() + half, which.end()), proof_of, rng, verdicts);
   }
 
   void verify_batch(size_t n, const uint64_t* const* inputs, const size_t* n_inputs, const uint8_t* const* proofs, const size_t* lens, b2m_rng* rng,
@@ -399,8 +446,7 @@ struct MarlinVerifier : VerifierBase {
     }
     // 2. decode on the GPU, straight into the MSM base array behind the shared bases
     Batch B;
-    B.n_bases = shared.size() + n_pts;
-    DBuf<Pt> bases(cx, B.n_bases);
+    DBuf<Pt> bases(cx, shared.size() + n_pts);
     std::vector<Pt> host_pts(n_pts);
     std::vector<int> status(n_pts);
     bases.upload(shared.data(), shared.size());
@@ -437,22 +483,23 @@ struct MarlinVerifier : VerifierBase {
         });
       for (auto& th : pool) th.join();
     }
-    std::vector<size_t> live, proof_of;
+    std::vector<size_t> proof_of;
     for (size_t i = 0; i < n; i++) {
       if (!has_eq[i]) continue;  // verdict -1 (malformed) or 0 (no shifted commitment for a bounded polynomial)
-      live.push_back(B.eqs.size());
       proof_of.push_back(i);
       B.eqs.push_back(std::move(eqs[i]));
+      B.pt_lo.push_back(first[i] - shared.size());
+      B.pt_hi.push_back(first[i] - shared.size() + parsed[i].pt_off.size());
     }
     const double ms_transcript = ms_since(t0);
     // 4. + 5.
     double ms_tables = 0, ms_checks = 0;
-    if (!live.empty()) {
+    if (!B.eqs.empty()) {
       t0 = Clock::now();
-      B.msm.reset(new Msm<Fr, Fq>(cx, bases.p, B.n_bases, nullptr, 0, 0, true));
+      B.msm.reset(new Msm<Fr, Fq>(cx, bases.p + shared.size(), n_pts, shared.data(), shared.size(), 0, true));
       ms_tables = ms_since(t0);
       t0 = Clock::now();
-      resolve(B, live, proof_of, zr, verdicts);
+      resolve(B, proof_of, zr, verdicts);
       ms_checks = ms_since(t0);
     }
     zr.commit_position();

@@ -10,6 +10,7 @@ bisection.  The phase split is the library's own (host wall clock around synchro
 """
 import argparse
 import json
+import random
 import os
 import subprocess
 import sys
@@ -17,7 +18,7 @@ import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from marlin_b200 import api, r1cs  # noqa: E402
+from marlin_b200 import api, fields, r1cs  # noqa: E402
 
 
 def gpu_card():
@@ -39,9 +40,13 @@ def main():
     ap.add_argument("--pc", default="marlin_kzg10", choices=["marlin_kzg10", "sonic_kzg10"])
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=1)
+    ap.add_argument("--bad", type=int, default=0, help="proofs checked against a wrong public input, at seeded positions")
+    ap.add_argument("--seed", type=int, default=1, help="seed of the bad positions")
     args = ap.parse_args()
     if args.steps < 1 or args.batch < 1:
         ap.error("--steps and --batch must be at least 1")
+    if not 0 <= args.bad <= args.batch:
+        ap.error("--bad must be between 0 and --batch")
 
     m = api.Marlin(args.curve, args.pc, device=0)
     n = 1 << args.log_n
@@ -56,13 +61,17 @@ def main():
     distinct = [m.prove(pk, circ, api.ZkRng(bytes([i]) * 32, 12)) for i in range(64)]
     proofs = [distinct[i % 64] for i in range(args.batch)]
     inputs = [circ.public_input()] * len(proofs)
+    bad = set(random.Random(args.seed).sample(range(args.batch), args.bad))
+    wrong = [(x + 1) % fields.FR_MODULUS[m.curve_id] for x in circ.public_input()]
+    inputs = [wrong if i in bad else x for i, x in enumerate(inputs)]
+    want = [i not in bad for i in range(args.batch)]
     rng = api.ZkRng()
     for _ in range(max(args.warmup, 1)):
-        assert all(v is True for v in m.verify_batch(vk, inputs, proofs, rng))
+        assert m.verify_batch(vk, inputs, proofs, rng) == want
     secs, phases, ok = [], [], True
     for _ in range(args.steps):
         t0 = time.perf_counter()
-        ok = all(v is True for v in m.verify_batch(vk, inputs, proofs, rng)) and ok  # synchronous at return
+        ok = m.verify_batch(vk, inputs, proofs, rng) == want and ok  # synchronous at return
         secs.append(time.perf_counter() - t0)
         phases.append(vk.timings())
     keys = [k for k in phases[0] if k.endswith("_ms")]
@@ -71,7 +80,7 @@ def main():
         "metric": "verified_proofs_per_sec", "value": args.batch / mean_s, "unit": "proofs/s", "n_gpus": 1, "steps": args.steps,
         "warmup": max(args.warmup, 1), "ms_per_batch": 1e3 * mean_s, "higher_is_better": True,
         "config": {"workload": f"Marlin.verify_batch of {args.batch} proofs (64 distinct, repeated) of DummyCircuit 2^{args.log_n}, "
-                               f"{args.curve}, {args.pc}",
+                               f"{args.curve}, {args.pc}, {args.bad} checked against a wrong public input (seed {args.seed})",
                    "timing": "host wall clock around each verify_batch call (synchronous at return)"},
         "all_accepted": ok, "phases_ms": {k: sum(p[k] for p in phases) / len(phases) for k in keys}, "checks_per_batch": phases[-1]["checks"],
         "gpu": gpu_card(),
