@@ -140,5 +140,8 @@ extern "C" {
                             proofs: *const *const u8, proof_lens: *const usize, rng: *mut b2m_rng, verdicts: *mut c_int) -> c_int;
     pub fn b2m_verify(vk: *mut b2m_vk, public_input: *const u64, n_input: usize, proof: *const u8, proof_len: usize,
                       rng: *mut b2m_rng, ok: *mut c_int) -> c_int;
+    pub fn b2m_verify_multi(n_keys: usize, vks: *const *mut b2m_vk, n: usize, key_of: *const u32, public_inputs: *const *const u64,
+                            n_inputs: *const usize, proofs: *const *const u8, proof_lens: *const usize, rng: *mut b2m_rng,
+                            verdicts: *mut c_int) -> c_int;
     pub fn b2m_verify_timings(vk: *const b2m_vk, json: *mut c_char, cap: usize) -> c_int;
 }

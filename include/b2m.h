@@ -413,8 +413,21 @@ int b2m_verify_batch(b2m_vk* vk, size_t n, const uint64_t* const* public_inputs,
 /* A batch of one: *ok receives the verdict (1, 0 or -1). */
 int b2m_verify(b2m_vk* vk, const uint64_t* public_input, size_t n_input, const uint8_t* proof, size_t proof_len,
                b2m_rng* rng, int* ok);
-/* Phase split of the last b2m_verify_batch on this key (host wall-clock milliseconds around synchronised work):
- * {"decode_ms", "transcript_ms", "msm_tables_ms", "msm_ms", "pairing_ms", "first_check_ms", "bisection_ms", "checks", ...}. */
+/* `Marlin::verify` for n proofs under n_keys verifier keys at once.  Proof i is checked under vks[key_of[i]].  All keys must
+ * belong to the same b2m_ctx and curve; PC variants and SRSs may differ, and a key may appear more than once.  Verdicts, rng
+ * requirements and malformed-proof handling are those of b2m_verify_batch; verdicts[i] equals what
+ * b2m_verify_batch(vks[key_of[i]], ...) gives proof i.  Keys whose SRSs share h and beta h share one G2 group: every check
+ * folds all its proofs into one set of MSMs and decides one pairing product per G2 group, all products of a bisection level
+ * in one launch.  Randomisers are drawn as b2m_verify_batch draws them, in item order, so one key gives exactly its draws.
+ * A null key, keys of two contexts or curves and key_of[i] >= n_keys fail with B2M_ERR_INVALID_ARG naming the index, before
+ * any work or rng draw; rng as b2m_verify_batch.  n = 0 is allowed.  The call's timings go to every key in vks. */
+int b2m_verify_multi(size_t n_keys, b2m_vk* const* vks, size_t n, const uint32_t* key_of,
+                     const uint64_t* const* public_inputs, const size_t* n_inputs, const uint8_t* const* proofs,
+                     const size_t* proof_lens, b2m_rng* rng, int* verdicts);
+/* Phase split of the last b2m_verify_batch or b2m_verify_multi on this key (host wall-clock milliseconds around synchronised
+ * work): {"decode_ms", "transcript_ms", "g2_set_ms", "msm_tables_ms", "msm_ms", "pairing_ms", "first_check_ms",
+ * "bisection_ms", "checks", "keys", "g2_groups", "products", ...}.  g2_set_ms: assembling the call's G2 set from the keys'
+ * prepared lines; keys: distinct keys of the call; products: pairing products over all checks. */
 int b2m_verify_timings(const b2m_vk* vk, char* json, size_t cap);
 
 #ifdef __cplusplus

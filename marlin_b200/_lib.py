@@ -126,6 +126,7 @@ def lib():
             L.b2m_vk_destroy.restype = None
             L.b2m_verify_batch.argtypes = [vp, sz, vp, vp, vp, vp, P(Rng), vp]
             L.b2m_verify.argtypes = [vp, vp, sz, vp, sz, P(Rng), P(ci)]
+            L.b2m_verify_multi.argtypes = [sz, vp, sz, vp, vp, vp, vp, vp, P(Rng), vp]
             L.b2m_verify_timings.argtypes = [vp, ctypes.c_char_p, sz]
         _lib = L
     return _lib

@@ -441,6 +441,40 @@ def domain_bytes(cid, size):
     return out.tobytes()
 
 
+def _proof_args(curve_ids, public_inputs, proofs):
+    """b2m_verify_batch / b2m_verify_multi arguments for proof i of curve curve_ids[i]: (input pointers, input lengths, proof
+    pointers, proof lengths), the verdict array, and the buffers behind the pointers (kept alive by the caller)"""
+    n = len(proofs)
+    ins = [np.ascontiguousarray(_lib.ints_to_limbs([fields.fr_to_mont(c, v % fields.FR_MODULUS[c]) for v in x], 4))
+           for c, x in zip(curve_ids, public_inputs)]
+    bufs = [np.frombuffer(bytes(p), dtype=np.uint8).copy() if len(p) else np.zeros(1, dtype=np.uint8) for p in proofs]
+    in_ptrs = (ctypes.c_void_p * max(n, 1))(*[a.ctypes.data for a in ins])
+    in_lens = (ctypes.c_size_t * max(n, 1))(*[len(a) for a in ins])
+    pr_ptrs = (ctypes.c_void_p * max(n, 1))(*[a.ctypes.data for a in bufs])
+    pr_lens = (ctypes.c_size_t * max(n, 1))(*[len(p) for p in proofs])
+    return (in_ptrs, in_lens, pr_ptrs, pr_lens), (ctypes.c_int * max(n, 1))(), (ins, bufs)
+
+
+def verify_many(entries, rng):
+    """`Marlin::verify` for proofs under many verifier keys in one batch (b2m_verify_multi).  entries: (vk, public_input,
+    proof_bytes) triples, public inputs as `Marlin.verify_batch` takes them; the keys (collected by identity) must share one
+    Context and curve, their PC variants and SRSs may differ.  Returns True / False / None per entry: what
+    `verify_batch(vk, ...)` gives that entry under its own key.  rng: as for `verify_batch`."""
+    keys, key_of = [], []
+    for vk, _, _ in entries:
+        k = next((j for j, x in enumerate(keys) if x is vk), None)
+        if k is None:
+            k = len(keys)
+            keys.append(vk)
+        key_of.append(k)
+    n = len(entries)
+    args, verdicts, _keep = _proof_args([keys[k].curve_id for k in key_of], [e[1] for e in entries], [e[2] for e in entries])
+    vks = (ctypes.c_void_p * max(len(keys), 1))(*[k.handle for k in keys])
+    kof = (ctypes.c_uint32 * max(n, 1))(*key_of)
+    _lib.check(_lib.lib().b2m_verify_multi(len(keys), vks, n, kof, *args, ctypes.byref(rng.c) if rng is not None else None, verdicts))
+    return [{1: True, 0: False}.get(verdicts[i]) for i in range(n)]
+
+
 def max_degree(num_constraints, num_variables, num_non_zero):
     """`AHPForR1CS::max_degree` [reference src/ahp/mod.rs:71-93]"""
     def p2(n):
@@ -935,16 +969,8 @@ class Marlin:
         n = len(proofs)
         if len(public_inputs) != n:
             raise ValueError("one public input per proof")
-        r = fields.FR_MODULUS[self.curve_id]
-        ins = [np.ascontiguousarray(_lib.ints_to_limbs([fields.fr_to_mont(self.curve_id, v % r) for v in x], 4)) for x in public_inputs]
-        bufs = [np.frombuffer(bytes(p), dtype=np.uint8).copy() if len(p) else np.zeros(1, dtype=np.uint8) for p in proofs]
-        in_ptrs = (ctypes.c_void_p * max(n, 1))(*[a.ctypes.data for a in ins])
-        in_lens = (ctypes.c_size_t * max(n, 1))(*[len(a) for a in ins])
-        pr_ptrs = (ctypes.c_void_p * max(n, 1))(*[a.ctypes.data for a in bufs])
-        pr_lens = (ctypes.c_size_t * max(n, 1))(*[len(p) for p in proofs])
-        verdicts = (ctypes.c_int * max(n, 1))()
-        _lib.check(_lib.lib().b2m_verify_batch(vk.handle, n, in_ptrs, in_lens, pr_ptrs, pr_lens,
-                                               ctypes.byref(rng.c) if rng is not None else None, verdicts))
+        args, verdicts, _keep = _proof_args([self.curve_id] * n, public_inputs, proofs)
+        _lib.check(_lib.lib().b2m_verify_batch(vk.handle, n, *args, ctypes.byref(rng.c) if rng is not None else None, verdicts))
         return [{1: True, 0: False}.get(verdicts[i]) for i in range(n)]
 
     def verify(self, vk, public_input, proof_bytes, rng):

@@ -742,8 +742,17 @@ int b2m_prove_timings(const b2m_index* idx, char* json, size_t cap) {
 // ---- Level 2: verifier ----------------------------------------------------------------------------
 struct b2m_vk {
   b2m_ctx* ctx;
+  int curve;
   std::unique_ptr<VerifierBase> impl;
 };
+
+// the batch randomisers must be unpredictable to the prover: a verify call without a usable rng is refused
+static void require_verify_rng(const b2m_rng* rng) {
+  B2M_REQUIRE(rng != nullptr, B2M_ERR_MISSING_RNG, "rng is required (the batch randomisers must be unpredictable to the prover)");
+  B2M_REQUIRE(rng->kind == B2M_RNG_CHACHA8 || rng->kind == B2M_RNG_CHACHA12 || rng->kind == B2M_RNG_CHACHA20 ||
+                  (rng->kind == B2M_RNG_CALLBACK && rng->next_u64 != nullptr),
+              B2M_ERR_MISSING_RNG, "unsupported rng kind %d", rng->kind);
+}
 
 int b2m_vk_create(b2m_ctx* ctx, int curve, int pc_variant, size_t num_constraints, size_t num_variables, size_t num_non_zero,
                   const uint64_t* index_comms_xy, const uint64_t* g_xy, const uint64_t* gamma_g_xy, const uint8_t* h_bytes,
@@ -757,7 +766,7 @@ int b2m_vk_create(b2m_ctx* ctx, int curve, int pc_variant, size_t num_constraint
     ctx->cx.use();
     const VkArgs a{pc_variant, num_constraints, num_variables, num_non_zero, index_comms_xy, g_xy, gamma_g_xy, h_bytes, beta_h_bytes,
                    n_bounds, bounds, bound_points};
-    std::unique_ptr<b2m_vk> vk(new b2m_vk{ctx, nullptr});
+    std::unique_ptr<b2m_vk> vk(new b2m_vk{ctx, curve, nullptr});
     const auto make = curve == B2M_CURVE_BLS12_381 ? make_verifier_bls : curve == B2M_CURVE_BN254 ? make_verifier_bn : make_verifier_bls377;
     vk->impl.reset(make(ctx->cx, a));
     *out = vk.release();
@@ -778,13 +787,31 @@ int b2m_verify_batch(b2m_vk* vk, size_t n, const uint64_t* const* public_inputs,
                      const size_t* proof_lens, b2m_rng* rng, int* verdicts) {
   return guard([&] {
     B2M_REQUIRE(vk && (n == 0 || (public_inputs && n_inputs && proofs && proof_lens && verdicts)), B2M_ERR_INVALID_ARG, "null argument");
-    B2M_REQUIRE(rng != nullptr, B2M_ERR_MISSING_RNG, "rng is required (the batch randomisers must be unpredictable to the prover)");
-    B2M_REQUIRE(rng->kind == B2M_RNG_CHACHA8 || rng->kind == B2M_RNG_CHACHA12 || rng->kind == B2M_RNG_CHACHA20 ||
-                    (rng->kind == B2M_RNG_CALLBACK && rng->next_u64 != nullptr),
-                B2M_ERR_MISSING_RNG, "unsupported rng kind %d", rng->kind);
+    require_verify_rng(rng);
     for (size_t i = 0; i < n; i++) B2M_REQUIRE(public_inputs[i] || n_inputs[i] == 0, B2M_ERR_INVALID_ARG, "public input %zu is null", i);
     vk->ctx->cx.use();
     vk->impl->verify_batch(n, public_inputs, n_inputs, proofs, proof_lens, rng, verdicts);
+  });
+}
+
+int b2m_verify_multi(size_t n_keys, b2m_vk* const* vks, size_t n, const uint32_t* key_of, const uint64_t* const* public_inputs,
+                     const size_t* n_inputs, const uint8_t* const* proofs, const size_t* proof_lens, b2m_rng* rng, int* verdicts) {
+  return guard([&] {
+    B2M_REQUIRE((n_keys == 0 || vks) && (n == 0 || (key_of && public_inputs && n_inputs && proofs && proof_lens && verdicts)), B2M_ERR_INVALID_ARG,
+                "null argument");
+    for (size_t k = 0; k < n_keys; k++) {
+      B2M_REQUIRE(vks[k], B2M_ERR_INVALID_ARG, "key %zu is null", k);
+      B2M_REQUIRE(vks[k]->ctx == vks[0]->ctx, B2M_ERR_INVALID_ARG, "key %zu belongs to another context than key 0", k);
+      B2M_REQUIRE(vks[k]->curve == vks[0]->curve, B2M_ERR_INVALID_ARG, "key %zu is on curve %d, key 0 on curve %d", k, vks[k]->curve, vks[0]->curve);
+    }
+    for (size_t i = 0; i < n; i++) B2M_REQUIRE(key_of[i] < n_keys, B2M_ERR_INVALID_ARG, "key_of[%zu] = %u is not below n_keys = %zu", i, key_of[i], n_keys);
+    require_verify_rng(rng);
+    for (size_t i = 0; i < n; i++) B2M_REQUIRE(public_inputs[i] || n_inputs[i] == 0, B2M_ERR_INVALID_ARG, "public input %zu is null", i);
+    if (n_keys == 0) return;  // (and so n == 0)
+    std::vector<VerifierBase*> impls(n_keys);
+    for (size_t k = 0; k < n_keys; k++) impls[k] = vks[k]->impl.get();
+    vks[0]->ctx->cx.use();
+    impls[0]->verify_multi(n_keys, impls.data(), n, key_of, public_inputs, n_inputs, proofs, proof_lens, rng, verdicts);
   });
 }
 

@@ -68,6 +68,20 @@ struct PairingG2Set {
     inf.upload(hinf.data(), hinf.size());
   }
 
+  // points of sets prepared before: point i is point src[i].second of set *src[i].first, its lines copied on the device (runs of
+  // consecutive points of one set in one copy) rather than computed again
+  PairingG2Set(Ctx& c, const std::vector<std::pair<const PairingG2Set*, size_t>>& src) : cx(c), n(src.size()), C(src.at(0).first->C) {
+    lines = DBuf<G2Line<Fq>>(cx, n * NL);
+    inf = DBuf<uint8_t>(cx, n);
+    for (size_t i = 0, j; i < n; i = j) {
+      const PairingG2Set* s = src[i].first;
+      const size_t q = src[i].second;
+      for (j = i + 1; j < n && src[j].first == s && src[j].second == q + (j - i);) j++;
+      B2M_CUDA(cudaMemcpyAsync(lines.p + i * NL, s->lines.p + q * NL, (j - i) * NL * sizeof(G2Line<Fq>), cudaMemcpyDeviceToDevice, cx.stream));
+      B2M_CUDA(cudaMemcpyAsync(inf.p + i, s->inf.p + q, j - i, cudaMemcpyDeviceToDevice, cx.stream));
+    }
+  }
+
   // verdicts[k] = (product k == 1), product k being the pairs [off[k], off[k + 1]) of (g1_xy[j], G2 point g2_index[j]).
   // B2M_ERR_INVALID_ARG for malformed offsets or indices and, naming the pair, for a G1 point off the curve.
   void check(size_t n_products, const size_t* off, const uint64_t* g1_xy, const uint32_t* g2_index, int* verdicts) {

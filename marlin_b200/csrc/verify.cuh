@@ -9,9 +9,17 @@ namespace b2m {
 
 struct VerifierBase {
   virtual ~VerifierBase() {}
-  // `Marlin::verify` [reference src/lib.rs:315-433] for n proofs under this key; verdicts[i] = 1 / 0 / -1 (malformed)
-  virtual void verify_batch(size_t n, const uint64_t* const* public_inputs, const size_t* n_inputs, const uint8_t* const* proofs,
-                            const size_t* proof_lens, b2m_rng* rng, int* verdicts) = 0;
+  // `Marlin::verify` [reference src/lib.rs:315-433] for n proofs, proof i under keys[key_of[i]] (keys of this key's curve and
+  // context, repeats allowed); verdicts[i] = 1 / 0 / -1 (malformed).  Every key of the call gets its timings_json.
+  virtual void verify_multi(size_t n_keys, VerifierBase* const* keys, size_t n, const uint32_t* key_of, const uint64_t* const* public_inputs,
+                            const size_t* n_inputs, const uint8_t* const* proofs, const size_t* proof_lens, b2m_rng* rng, int* verdicts) = 0;
+  // n proofs under this key: the one-key case of verify_multi
+  void verify_batch(size_t n, const uint64_t* const* public_inputs, const size_t* n_inputs, const uint8_t* const* proofs,
+                    const size_t* proof_lens, b2m_rng* rng, int* verdicts) {
+    VerifierBase* self = this;
+    const std::vector<uint32_t> key_of(n, 0);
+    verify_multi(1, &self, n, key_of.data(), public_inputs, n_inputs, proofs, proof_lens, rng, verdicts);
+  }
   std::string timings_json;
 };
 

@@ -1,4 +1,5 @@
-// Batched `Marlin::verify` [reference src/lib.rs:315-433] for one index verifier key.
+// Batched `Marlin::verify` [reference src/lib.rs:315-433] for proofs under one or more index verifier keys of one curve.
+// MarlinVerifier holds one key's data; VerifyItems checks a batch of (key, proof) items, b2m_verify_batch being its one-key case.
 //
 //   1. parse (host)        the `Proof` CanonicalDeserialize framing; evaluations and random_v must be canonical Fr
 //   2. decode (GPU)        one thread per compressed G1 point of the whole batch (g1_decode.cuh): flags, x < p, square root,
@@ -7,9 +8,12 @@
 //                          bookkeeping of the PC scheme -> per proof and point a list of (Fr scalar, G1 base) terms of
 //                              e(plain + z W, h) * e(-W, beta h) * prod_d e(C_d, beta^-(D-d) h) = 1
 //   4. batch check         one 128-bit randomiser per (proof, point) from the caller's rng folds every equation into
-//                          MSM_A (plain + z W), MSM_B (W) and, for SonicKZG10, one MSM per bound -- over the checked proofs'
-//                          slice of the device-resident bases plus the shared bases (index commitments, g, gamma g, shift
-//                          powers) with summed scalars -- and one pairing product, checked on the GPU (pairing_impl.cuh)
+//                          MSM_A (plain + z W), MSM_B (W) and, for SonicKZG10, one MSM per bound point -- over the checked
+//                          proofs' slice of the device-resident bases plus every key's shared bases (index commitments, g,
+//                          gamma g, shift powers) with summed scalars -- and one pairing product, checked on the GPU
+//                          (pairing_impl.cuh).  Keys with equal (h, beta h) form one G2 group (verify_layout.hpp) with its own
+//                          A and B MSMs and its own product; a check passes iff all its products are 1.  The G1 terms under
+//                          different keys are independent, so independent randomisers keep the folded check sound.
 //   5. bisection           a failing set is split in halves, each checked with fresh randomisers, until every bad proof is
 //                          isolated: m bad proofs cost O(m log N) extra checks, made level by level (all checks of a level in
 //                          one MSM batch and one pairing launch), so O(log N) rounds
@@ -26,6 +30,7 @@
 #include "pairing_impl.cuh"
 #include "prover_impl.cuh"  // MarlinIndex's ToBytes writers (the transcript encodes commitments as the prover does)
 #include "verify.cuh"
+#include "verify_layout.hpp"
 
 namespace b2m {
 
@@ -51,10 +56,11 @@ struct MarlinVerifier : VerifierBase {
   Ctx& cx;
   int pc;
   size_t nc, nv, nnz, H, K;
-  std::vector<Pt> shared;  // bases 0 .. shared.size()
+  std::vector<Pt> shared;  // this key's shared bases, at a per-call offset among the MSM's extra bases
   std::vector<uint64_t> bounds;
   size_t bidx_h, bidx_k;  // indices of |H| - 2 and |K| - 2 among the bounds
-  std::unique_ptr<PairingG2Set<Fq>> g2set;  // h, beta_h, then SonicKZG10's beta^-(D - d) h per bound, prepared for the GPU pairing
+  std::vector<uint8_t> g2_bytes;            // h, beta_h, then SonicKZG10's beta^-(D - d) h per bound (uncompressed)
+  std::unique_ptr<PairingG2Set<Fq>> g2set;  // the same points, prepared for the GPU pairing
   std::vector<uint8_t> vk_bytes;
 
   static size_t pow2_at_least(size_t n) {
@@ -96,17 +102,20 @@ struct MarlinVerifier : VerifierBase {
                     "neg_powers_of_h[%zu] is not a finite point of the G2 curve", k);
       }
     }
-    std::vector<uint8_t> g2b(a.h_bytes, a.h_bytes + 4 * FQ_BYTES);
-    g2b.insert(g2b.end(), a.beta_h_bytes, a.beta_h_bytes + 4 * FQ_BYTES);
+    g2_bytes.assign(a.h_bytes, a.h_bytes + 4 * FQ_BYTES);
+    g2_bytes.insert(g2_bytes.end(), a.beta_h_bytes, a.beta_h_bytes + 4 * FQ_BYTES);
     if (pc == B2M_PC_SONIC_KZG10)
-      g2b.insert(g2b.end(), static_cast<const uint8_t*>(a.bound_points), static_cast<const uint8_t*>(a.bound_points) + a.n_bounds * 4 * FQ_BYTES);
-    g2set.reset(new PairingG2Set<Fq>(cx, g2b.size() / (4 * FQ_BYTES), g2b.data()));
+      g2_bytes.insert(g2_bytes.end(), static_cast<const uint8_t*>(a.bound_points),
+                      static_cast<const uint8_t*>(a.bound_points) + a.n_bounds * 4 * FQ_BYTES);
+    g2set.reset(new PairingG2Set<Fq>(cx, g2_points(), g2_bytes.data()));
     // IndexVerifierKey ToBytes [reference src/data_structures.rs:36-43]: index_info || index_comms
     put_u64(vk_bytes, nv);
     put_u64(vk_bytes, nc);
     put_u64(vk_bytes, nnz);
     for (int i = 0; i < 6; i++) write_commitment(vk_bytes, shared[i], false, Pt::inf());
   }
+
+  size_t g2_points() const { return g2_bytes.size() / (4 * FQ_BYTES); }
 
   void write_commitment(std::vector<uint8_t>& out, const Pt& comm, bool has_shifted, const Pt& shifted) const {
     MI::put_affine_tobytes(out, comm);
@@ -214,8 +223,9 @@ struct MarlinVerifier : VerifierBase {
     return Fr::from_canonical(c);
   }
 
-  // false: the proof is rejected without a pairing (a degree-bounded commitment without its shifted half)
-  bool equations(const Parsed& P, const Pt* pts, uint32_t base0, const uint64_t* input, size_t n_input, ProofEq& E) const {
+  // false: the proof is rejected without a pairing (a degree-bounded commitment without its shifted half).  The proof's points
+  // are bases base0 + slot, this key's shared bases sbase0 + S_*.
+  bool equations(const Parsed& P, const Pt* pts, uint32_t base0, uint32_t sbase0, const uint64_t* input, size_t n_input, ProofEq& E) const {
     const bool marlin = pc == B2M_PC_MARLIN_KZG10;
     if (marlin && (P.shifted[C_G1] < 0 || P.shifted[C_G2] < 0)) return false;
     const Fr one = Fr::one();
@@ -293,7 +303,7 @@ struct MarlinVerifier : VerifierBase {
         pe.plain.push_back(Term{c0, base(P.comm[comm])});
         const Fr c1 = next();  // c1 (shifted - v powers_of_g[D - d])
         pe.plain.push_back(Term{c1, base(P.shifted[comm])});
-        pe.plain.push_back(Term{(c1 * v).neg(), (uint32_t)(S_SHIFT + bidx)});
+        pe.plain.push_back(Term{(c1 * v).neg(), sbase0 + (uint32_t)(S_SHIFT + bidx)});
       };
       auto plain_lc = [&](std::initializer_list<std::pair<Fr, uint32_t>> terms, Fr v) {
         const Fr c = next();
@@ -309,69 +319,104 @@ struct MarlinVerifier : VerifierBase {
       } else {  // gamma: g_2, inner_sumcheck
         pe.z = gamma;
         bounded_lc(C_G2, g2_g, bidx_k);
-        plain_lc({{eta_a * vv, S_AVAL}, {eta_b * vv, S_BVAL}, {eta_c * vv, S_CVAL}, {bscale * alpha, S_ROW}, {bscale * beta, S_COL},
-                  {bscale.neg(), S_ROWCOL}, {v_k_gamma.neg(), base(P.comm[C_H2])}},
+        plain_lc({{eta_a * vv, sbase0 + S_AVAL}, {eta_b * vv, sbase0 + S_BVAL}, {eta_c * vv, sbase0 + S_CVAL}, {bscale * alpha, sbase0 + S_ROW},
+                  {bscale * beta, sbase0 + S_COL}, {bscale.neg(), sbase0 + S_ROWCOL}, {v_k_gamma.neg(), base(P.comm[C_H2])}},
                  v_inner);
       }
-      pe.plain.push_back(Term{combined.neg(), S_G});
-      if (P.has_rv[j]) pe.plain.push_back(Term{P.rv[j].neg(), S_GAMMA_G});
+      pe.plain.push_back(Term{combined.neg(), sbase0 + S_G});
+      if (P.has_rv[j]) pe.plain.push_back(Term{P.rv[j].neg(), sbase0 + S_GAMMA_G});
       pe.w = base(P.w[j]);
     }
     return true;
   }
 
-  // ---- 4. + 5. randomised checks, the bisection tree level by level ---------------------------------------------------
-  struct Batch {
-    std::unique_ptr<Msm<Fr, Fq>> msm;  // bases: the proofs' points; extra bases: the shared ones
-    std::vector<ProofEq> eqs;
-    std::vector<size_t> pt_lo, pt_hi;  // per equation: its proof's points [lo, hi) among the proof points
-    double ms_msm = 0, ms_pairing = 0, ms_first = 0;
-    int checks = 0;
-  };
+  void verify_multi(size_t n_keys, VerifierBase* const* keys, size_t n, const uint32_t* key_of, const uint64_t* const* inputs,
+                    const size_t* n_inputs, const uint8_t* const* proofs, const size_t* lens, b2m_rng* rng, int* verdicts) override;
+};
+
+// ---- 4. + 5. randomised checks, the bisection tree level by level ---------------------------------------------------------
+template <class Fr, class Fq>
+struct VerifyItems {
+  using V = MarlinVerifier<Fr, Fq>;
+  using Pt = Affine<Fq>;
   using Clock = std::chrono::steady_clock;
   static double ms_since(Clock::time_point t) { return std::chrono::duration<double, std::milli>(Clock::now() - t).count(); }
 
-  // A node is a range [a, b) of equations (contiguous in proof order, so its proofs' points are one slice of the bases).
-  // The root is checked; a failing node of one proof is a bad proof, a failing larger node has both halves checked.  That is
-  // the depth-first bisection's set of checks, with the same randomisers per check (two 128-bit ones per proof), so the rng
-  // ends at the same position; they are only drawn level by level.  All checks of a level run their MSMs as one
-  // Msm::run_batch sequence (each MSM over its node's slice plus the shared bases) and their pairing products as one
-  // PairingG2Set::check launch.
-  void resolve(Batch& B, const std::vector<size_t>& proof_of, ZkSource<b2m_rng>& rng, int* verdicts) const {
+  Ctx& cx;
+  std::vector<const V*> keys;  // the call's distinct keys
+  std::vector<uint32_t> sbase;  // per key: its first shared base
+  std::vector<Pt> shared;       // every key's shared bases, concatenated
+  std::unique_ptr<Msm<Fr, Fq>> msm;  // bases: the proofs' points; extra bases: the shared ones
+  std::vector<typename V::ProofEq> eqs;
+  std::vector<uint32_t> key;         // per equation: its key
+  std::vector<size_t> pt_lo, pt_hi;  // per equation: its proof's points [lo, hi) among the proof points
+  double ms_msm = 0, ms_pairing = 0, ms_first = 0;
+  int checks = 0, products = 0;
+
+  explicit VerifyItems(Ctx& c) : cx(c) {}
+
+  // A node is a range [a, b) of equations (contiguous in item order, so its proofs' points are one slice of the bases).  The
+  // root is checked; a failing node of one proof is a bad proof, a failing larger node has both halves checked.  That is the
+  // depth-first bisection's set of checks, with the same randomisers per check (two 128-bit ones per proof), so the rng ends at
+  // the same position; they are only drawn level by level.  A check has one pairing product per G2 group among its proofs:
+  // [A_g against h_g, -B_g against beta h_g, then group g's SonicKZG10 slots], and passes iff all of them are 1.  All checks
+  // of a level run their MSMs as one Msm::run_batch sequence (each MSM over its node's slice plus the shared bases) and their
+  // products as one PairingG2Set::check launch.
+  void resolve(const G2Layout& L, PairingG2Set<Fq>& g2, const std::vector<size_t>& proof_of, ZkSource<b2m_rng>& rng, int* verdicts) {
     const size_t S = shared.size();
-    std::vector<std::pair<size_t, size_t>> level{{0, B.eqs.size()}};
+    std::vector<std::pair<size_t, size_t>> level{{0, eqs.size()}};
+    std::vector<size_t> prod_of_group(L.n_groups), job_of_point(L.src.size());
     bool first = true;
     while (!level.empty()) {
       const Clock::time_point t_level = Clock::now();
       // scalars: per MSM, its node's slice (len values) then the S shared bases
       std::vector<Fr> sc;
       std::vector<size_t> job_off, job_len, job_lo;
-      std::vector<std::vector<std::pair<size_t, uint32_t>>> node_jobs(level.size());  // (job, G2 point) per pair
+      struct Pair {
+        size_t job;
+        uint32_t g2;
+        bool neg;  // -W against beta h
+      };
+      std::vector<std::vector<Pair>> prods;  // the level's products
+      std::vector<size_t> node_prod{0};      // node nd's products: [node_prod[nd], node_prod[nd + 1])
       for (size_t nd = 0; nd < level.size(); nd++) {
-        const size_t a = level[nd].first, b = level[nd].second, lo = B.pt_lo[a], len = B.pt_hi[b - 1] - lo;
-        auto new_job = [&](uint32_t g2) {
+        const size_t a = level[nd].first, b = level[nd].second, lo = pt_lo[a], len = pt_hi[b - 1] - lo;
+        auto new_job = [&]() {
           job_off.push_back(sc.size());
           job_len.push_back(len);
           job_lo.push_back(lo);
           sc.resize(sc.size() + len + S, Fr::zero());
-          node_jobs[nd].push_back({job_off.size() - 1, g2});
           return job_off.size() - 1;
         };
-        const size_t ja = new_job(0), jb = new_job(1);  // plain + z W against h, W against beta h
-        std::vector<size_t> jd(bounds.size(), SIZE_MAX);
         auto at = [&](size_t job, uint32_t base) -> Fr& { return base < S ? sc[job_off[job] + len + base] : sc[job_off[job] + (base - S - lo)]; };
-        for (size_t i = a; i < b; i++)
-          for (const PointEq& pe : B.eqs[i].pt) {
+        std::fill(prod_of_group.begin(), prod_of_group.end(), SIZE_MAX);
+        std::fill(job_of_point.begin(), job_of_point.end(), SIZE_MAX);
+        for (size_t i = a; i < b; i++) {
+          const std::vector<uint32_t>& kp = L.point[key[i]];
+          size_t& pg = prod_of_group[L.group[key[i]]];
+          if (pg == SIZE_MAX) {  // plain + z W against h, W against beta h
+            pg = prods.size();
+            const size_t ja = new_job(), jb = new_job();
+            prods.push_back({Pair{ja, kp[0], false}, Pair{jb, kp[1], true}});
+          }
+          const size_t ja = prods[pg][0].job, jb = prods[pg][1].job;
+          for (const auto& pe : eqs[i].pt) {
             uint64_t rlo = rng.next_u64(), rhi = rng.next_u64();
-            const Fr r = fr_u128(rlo, rhi);
-            for (const Term& t : pe.plain) at(ja, t.base) = at(ja, t.base) + r * t.c;
+            const Fr r = V::fr_u128(rlo, rhi);
+            for (const auto& t : pe.plain) at(ja, t.base) = at(ja, t.base) + r * t.c;
             at(ja, pe.w) = at(ja, pe.w) + r * pe.z;
             at(jb, pe.w) = at(jb, pe.w) + r;
             for (const auto& bt : pe.bounded) {
-              if (jd[bt.first] == SIZE_MAX) jd[bt.first] = new_job((uint32_t)(2 + bt.first));
-              at(jd[bt.first], bt.second.base) = at(jd[bt.first], bt.second.base) + r * bt.second.c;
+              const uint32_t q = kp[2 + bt.first];
+              if (job_of_point[q] == SIZE_MAX) {
+                job_of_point[q] = new_job();
+                prods[pg].push_back(Pair{job_of_point[q], q, false});
+              }
+              at(job_of_point[q], bt.second.base) = at(job_of_point[q], bt.second.base) + r * bt.second.c;
             }
           }
+        }
+        node_prod.push_back(prods.size());
       }
       Clock::time_point t0 = Clock::now();
       for (Fr& x : sc) x = x.to_canonical();
@@ -387,31 +432,32 @@ struct MarlinVerifier : VerifierBase {
           jobs[k] = MsmJob<Fr, Fq>{dsc.p + job_off[j], false, job_len[j], job_lo[j], dsc.p + job_off[j] + job_len[j], S, 0, nullptr, 0, nullptr,
                                    dres.p + j};
         }
-        B.msm->run_batch(jobs, m);
+        msm->run_batch(jobs, m);
       }
       std::vector<Pt> res(nj);
       dres.download(res.data(), nj);
-      B.ms_msm += ms_since(t0);
+      ms_msm += ms_since(t0);
       t0 = Clock::now();
       std::vector<Pt> g1;
       std::vector<uint32_t> g2i;
       std::vector<size_t> off{0};
-      for (size_t nd = 0; nd < level.size(); nd++) {
-        for (const auto& jq : node_jobs[nd]) {
-          const Pt& q = res[jq.first];
-          g1.push_back(jq.second == 1 ? Pt{q.x, q.y.neg()} : q);  // -W against beta h (infinity stays (0, 0))
-          g2i.push_back(jq.second);
+      for (const auto& pr : prods) {
+        for (const Pair& p : pr) {
+          const Pt& q = res[p.job];
+          g1.push_back(p.neg ? Pt{q.x, q.y.neg()} : q);  // (infinity stays (0, 0))
+          g2i.push_back(p.g2);
         }
         off.push_back(g1.size());
       }
-      std::vector<int> ok(level.size());
-      g2set->check(level.size(), off.data(), reinterpret_cast<const uint64_t*>(g1.data()), g2i.data(), ok.data());
-      B.ms_pairing += ms_since(t0);
-      B.checks += (int)level.size();
+      std::vector<int> ok(prods.size());
+      g2.check(prods.size(), off.data(), reinterpret_cast<const uint64_t*>(g1.data()), g2i.data(), ok.data());
+      ms_pairing += ms_since(t0);
+      checks += (int)level.size();
+      products += (int)prods.size();
       std::vector<std::pair<size_t, size_t>> next;
       for (size_t nd = 0; nd < level.size(); nd++) {
         const size_t a = level[nd].first, b = level[nd].second;
-        if (ok[nd] == 1) {
+        if (std::all_of(ok.begin() + node_prod[nd], ok.begin() + node_prod[nd + 1], [](int v) { return v == 1; })) {
           for (size_t i = a; i < b; i++) verdicts[proof_of[i]] = 1;
         } else if (b - a == 1) {
           verdicts[proof_of[a]] = 0;
@@ -421,54 +467,66 @@ struct MarlinVerifier : VerifierBase {
           next.push_back({a + half, b});
         }
       }
-      if (first) B.ms_first = ms_since(t_level);
+      if (first) ms_first = ms_since(t_level);
       first = false;
       level.swap(next);
     }
   }
 
-  void verify_batch(size_t n, const uint64_t* const* inputs, const size_t* n_inputs, const uint8_t* const* proofs, const size_t* lens, b2m_rng* rng,
-                    int* verdicts) override {
+  // proof i under call key key_of[i] of n_keys
+  void run(size_t n_keys, VerifierBase* const* vks, size_t n, const uint32_t* key_of, const uint64_t* const* inputs, const size_t* n_inputs,
+           const uint8_t* const* proofs, const size_t* lens, b2m_rng* rng, int* verdicts) {
+    constexpr size_t FQ_BYTES = V::FQ_BYTES;
     Clock::time_point t_all = Clock::now(), t0 = t_all;
     ZkSource<b2m_rng> zr(rng);
+    // the distinct keys and their shared bases
+    std::vector<uint32_t> uniq(n_keys);
+    for (size_t k = 0; k < n_keys; k++) {
+      const V* v = static_cast<const V*>(vks[k]);
+      uniq[k] = (uint32_t)(std::find(keys.begin(), keys.end(), v) - keys.begin());
+      if (uniq[k] < keys.size()) continue;
+      keys.push_back(v);
+      sbase.push_back((uint32_t)shared.size());
+      shared.insert(shared.end(), v->shared.begin(), v->shared.end());
+    }
+    const size_t S = shared.size();
     // 1. framing
-    std::vector<Parsed> parsed(n);
+    std::vector<typename V::Parsed> parsed(n);
     std::vector<uint32_t> first(n, 0);
     std::vector<uint8_t> bytes;
     size_t n_pts = 0;
     for (size_t i = 0; i < n; i++) {
       verdicts[i] = -1;
-      if (!proofs[i] || !parse(proofs[i], lens[i], parsed[i])) continue;
+      if (!proofs[i] || !keys[uniq[key_of[i]]]->parse(proofs[i], lens[i], parsed[i])) continue;
       verdicts[i] = 0;
-      first[i] = (uint32_t)(shared.size() + n_pts);
+      first[i] = (uint32_t)(S + n_pts);
       for (size_t off : parsed[i].pt_off) bytes.insert(bytes.end(), proofs[i] + off, proofs[i] + off + FQ_BYTES);
       n_pts += parsed[i].pt_off.size();
     }
     // 2. decode on the GPU, straight into the MSM base array behind the shared bases
-    Batch B;
-    DBuf<Pt> bases(cx, shared.size() + n_pts);
+    DBuf<Pt> bases(cx, S + n_pts);
     std::vector<Pt> host_pts(n_pts);
     std::vector<int> status(n_pts);
-    bases.upload(shared.data(), shared.size());
+    bases.upload(shared.data(), S);
     if (n_pts) {
       DBuf<uint8_t> dbytes(cx, bytes.size());
       DBuf<int> dstatus(cx, n_pts);
       dbytes.upload(bytes.data(), bytes.size());
-      g1_decode_kernel<Fq><<<div_up(n_pts, 128), 128, 0, cx.stream>>>(dbytes.p, n_pts, bases.p + shared.size(), dstatus.p);
+      g1_decode_kernel<Fq><<<div_up(n_pts, 128), 128, 0, cx.stream>>>(dbytes.p, n_pts, bases.p + S, dstatus.p);
       B2M_CHECK_LAUNCH();
       cx.launches++;
       dstatus.download(status.data(), n_pts);
-      B2M_CUDA(cudaMemcpyAsync(host_pts.data(), bases.p + shared.size(), n_pts * sizeof(Pt), cudaMemcpyDeviceToHost, cx.stream));
+      B2M_CUDA(cudaMemcpyAsync(host_pts.data(), bases.p + S, n_pts * sizeof(Pt), cudaMemcpyDeviceToHost, cx.stream));
       cx.sync();
     }
     const double ms_decode = ms_since(t0);
     // 3. transcript and equations
     t0 = Clock::now();
-    std::vector<ProofEq> eqs(n);
+    std::vector<typename V::ProofEq> all_eqs(n);
     std::vector<char> has_eq(n, 0);
     for (size_t i = 0; i < n; i++) {
       if (verdicts[i] < 0) continue;
-      const size_t p0 = first[i] - shared.size();
+      const size_t p0 = first[i] - S;
       for (size_t k = 0; k < parsed[i].pt_off.size(); k++)
         if (status[p0 + k] != G1_OK) verdicts[i] = -1;
     }
@@ -478,8 +536,10 @@ struct MarlinVerifier : VerifierBase {
       for (unsigned t = 0; t < nt; t++)
         pool.emplace_back([&, t] {
           for (size_t i = t; i < n; i += nt)
-            if (verdicts[i] == 0)
-              has_eq[i] = equations(parsed[i], host_pts.data() + (first[i] - shared.size()), first[i], inputs[i], n_inputs[i], eqs[i]);
+            if (verdicts[i] == 0) {
+              const uint32_t u = uniq[key_of[i]];
+              has_eq[i] = keys[u]->equations(parsed[i], host_pts.data() + (first[i] - S), first[i], sbase[u], inputs[i], n_inputs[i], all_eqs[i]);
+            }
         });
       for (auto& th : pool) th.join();
     }
@@ -487,28 +547,46 @@ struct MarlinVerifier : VerifierBase {
     for (size_t i = 0; i < n; i++) {
       if (!has_eq[i]) continue;  // verdict -1 (malformed) or 0 (no shifted commitment for a bounded polynomial)
       proof_of.push_back(i);
-      B.eqs.push_back(std::move(eqs[i]));
-      B.pt_lo.push_back(first[i] - shared.size());
-      B.pt_hi.push_back(first[i] - shared.size() + parsed[i].pt_off.size());
+      eqs.push_back(std::move(all_eqs[i]));
+      key.push_back(uniq[key_of[i]]);
+      pt_lo.push_back(first[i] - S);
+      pt_hi.push_back(first[i] - S + parsed[i].pt_off.size());
     }
     const double ms_transcript = ms_since(t0);
-    // 4. + 5.
-    double ms_tables = 0, ms_checks = 0;
-    if (!B.eqs.empty()) {
+    // 4. + 5., with the call's G2 set: every group's points, copied from the keys' prepared lines
+    std::vector<std::pair<const uint8_t*, size_t>> kg2;
+    for (const V* v : keys) kg2.push_back({v->g2_bytes.data(), v->g2_points()});
+    const G2Layout L = g2_layout(kg2, 4 * FQ_BYTES);
+    double ms_g2 = 0, ms_tables = 0, ms_checks = 0;
+    if (!eqs.empty()) {
       t0 = Clock::now();
-      B.msm.reset(new Msm<Fr, Fq>(cx, bases.p + shared.size(), n_pts, shared.data(), shared.size(), 0, true));
+      std::vector<std::pair<const PairingG2Set<Fq>*, size_t>> src;
+      for (const auto& s : L.src) src.push_back({keys[s.first]->g2set.get(), s.second});
+      PairingG2Set<Fq> g2(cx, src);
+      ms_g2 = ms_since(t0);
+      t0 = Clock::now();
+      msm.reset(new Msm<Fr, Fq>(cx, bases.p + S, n_pts, shared.data(), S, 0, true));
       ms_tables = ms_since(t0);
       t0 = Clock::now();
-      resolve(B, proof_of, zr, verdicts);
+      resolve(L, g2, proof_of, zr, verdicts);
       ms_checks = ms_since(t0);
     }
     zr.commit_position();
     // msm_ms / pairing_ms cover every check; bisection_ms is the time of the checks after the first
-    timings_json = fmt(
-        "{\"proofs\": %zu, \"points\": %zu, \"decode_ms\": %.4f, \"transcript_ms\": %.4f, \"msm_tables_ms\": %.4f, \"msm_ms\": %.4f, "
-        "\"pairing_ms\": %.4f, \"first_check_ms\": %.4f, \"bisection_ms\": %.4f, \"checks\": %d, \"total_ms\": %.4f}",
-        n, n_pts, ms_decode, ms_transcript, ms_tables, B.ms_msm, B.ms_pairing, B.ms_first, ms_checks - B.ms_first, B.checks, ms_since(t_all));
+    const std::string json = fmt(
+        "{\"proofs\": %zu, \"points\": %zu, \"decode_ms\": %.4f, \"transcript_ms\": %.4f, \"g2_set_ms\": %.4f, \"msm_tables_ms\": %.4f, "
+        "\"msm_ms\": %.4f, \"pairing_ms\": %.4f, \"first_check_ms\": %.4f, \"bisection_ms\": %.4f, \"checks\": %d, \"keys\": %zu, "
+        "\"g2_groups\": %zu, \"products\": %d, \"total_ms\": %.4f}",
+        n, n_pts, ms_decode, ms_transcript, ms_g2, ms_tables, ms_msm, ms_pairing, ms_first, ms_checks - ms_first, checks, keys.size(), L.n_groups,
+        products, ms_since(t_all));
+    for (size_t k = 0; k < n_keys; k++) vks[k]->timings_json = json;
   }
 };
+
+template <class Fr, class Fq>
+void MarlinVerifier<Fr, Fq>::verify_multi(size_t n_keys, VerifierBase* const* keys, size_t n, const uint32_t* key_of, const uint64_t* const* inputs,
+                                          const size_t* n_inputs, const uint8_t* const* proofs, const size_t* lens, b2m_rng* rng, int* verdicts) {
+  VerifyItems<Fr, Fq>(cx).run(n_keys, keys, n, key_of, inputs, n_inputs, proofs, lens, rng, verdicts);
+}
 
 }  // namespace b2m
