@@ -92,6 +92,12 @@ extern "C" {
                        out_has_random_v: *mut c_int, out_random_v: *mut u64) -> c_int;
     pub fn b2m_g1_powers(ctx: *mut b2m_ctx, curve: c_int, g_xy: *const u64, beta: *const u64, n: usize, out_powers_xy: *mut u64) -> c_int;
     pub fn b2m_fixed_base_msm(ctx: *mut b2m_ctx, curve: c_int, g_xy: *const u64, scalars: *const u64, n: usize, out_xy: *mut u64) -> c_int;
+    pub fn b2m_g1_decode_lem(ctx: *mut b2m_ctx, curve: c_int, bytes: *const u8, n: usize, out_xy: *mut u64, bad_index: *mut usize,
+                             bad_reason: *mut c_int) -> c_int;
+    pub fn b2m_g2_decode_lem(ctx: *mut b2m_ctx, curve: c_int, bytes: *const u8, n: usize, out_uncompressed: *mut u8, bad_index: *mut usize,
+                             bad_reason: *mut c_int) -> c_int;
+    pub fn b2m_srs_check_powers(srs: *mut b2m_srs, h: *const u8, beta_h: *const u8, n_neg: usize, neg_keys: *const u64, neg_h: *const u8,
+                                rng: *mut b2m_rng, ok: *mut c_int, bad_kind: *mut c_int, bad_index: *mut usize) -> c_int;
     pub fn b2m_pairing_check(ctx: *mut b2m_ctx, curve: c_int, n_g2: usize, g2: *const u8, n_products: usize, product_off: *const usize,
                              g1_xy: *const u64, g2_index: *const u32, verdicts: *mut c_int) -> c_int;
     pub fn b2m_trim(srs: *mut b2m_srs, pc_variant: c_int, supported_degree: usize, supported_hiding_bound: usize,

@@ -180,6 +180,16 @@ int b2m_g1_decode_ark(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, i
                       size_t* bad_index, int* bad_reason);
 int b2m_g2_decode_ark(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, int compressed, uint8_t* out_uncompressed,
                       size_t* bad_index, int* bad_reason);
+/* Checked decoding of snarkjs "LEM" points, the form of a Powers-of-Tau (.ptau) file: uncompressed, every Fq (every Fq2 component,
+ * c0 then c1) little-endian Montgomery limbs with R = 2^(64 * limbs), no flags, all-zero bytes = infinity.  Same checks,
+ * chunking and status contract as b2m_g1_decode_ark / b2m_g2_decode_ark: each coordinate limb vector < p (a non-reduced
+ * representative is invalid: 2 x, 5 y), the curve equation (3) and the prime-order subgroup (4).  Infinity decodes with status
+ * OK; callers that need a finite point check for it.  Any curve id is accepted.
+ *   G1: bytes = n * 2 sizeof(Fq); out_xy = n affine Montgomery points (infinity = 0, 0).
+ *   G2: bytes = n * 4 sizeof(Fq); out_uncompressed = n * 4 sizeof(Fq) canonical ark bytes (the b2m_vk_create form). */
+int b2m_g1_decode_lem(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, uint64_t* out_xy, size_t* bad_index, int* bad_reason);
+int b2m_g2_decode_lem(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, uint8_t* out_uncompressed, size_t* bad_index,
+                      int* bad_reason);
 /* `PairingEngine::product_of_pairings(pairs).is_one()` [U ark-ec 0.3] for many products at once.  g2: n_g2 distinct G2 points
  * as uncompressed ark-serialize bytes (the b2m_g2_scalar_muls / b2m_vk_create form).  Product k is the pairs
  * [product_off[k], product_off[k+1]): G1 point g1_xy[j] (affine Montgomery, (0,0) = infinity) with G2 point g2_index[j].
@@ -232,6 +242,21 @@ typedef struct {
   uint64_t (*next_u64)(void* state); /* B2M_RNG_CALLBACK only */
   void* state;
 } b2m_rng;
+
+/* Is the key one chain of powers?  With P_i = powers_of_g[i] (D = b2m_srs_size - 1), G_k the gamma power of key k held on the
+ * device and N_k = neg_h[j] for key k = neg_keys[j] (optional: SonicKZG10's beta^-k h), decides all of
+ *   (0) e(P_{i+1}, h) = e(P_i, beta_h)  for i < D          (1) e(G_{k+1}, h) = e(G_k, beta_h)  for held keys k, k + 1
+ *   (2) e(P_k, N_k)   = e(P_0, h)       for every neg key  (3) e(G_k, N_k)   = e(G_0, h)       for every neg key with G_k held
+ * h, beta_h and neg_h are uncompressed ark G2 bytes (b2m_g2_decode_ark / _lem output; their subgroup is the caller's check).
+ * One randomised check on the GPU -- two D-pair MSMs over the window tables, a few one-pair MSMs, one pairing product of
+ * 3 + n_neg pairs -- and, when it fails, bisection with fresh randomisers.  *ok = 1 when every relation holds; otherwise *ok = 0,
+ * *bad_kind = the family (0-3) and *bad_index = i (family 0) or the key k of the lowest failing relation of the first failing
+ * family.  A bad relation passes a check with probability at most 2^-128.  Randomisers: two next_u64() per relation and check,
+ * family 0 in ascending i (ChaCha: generated on the device at the stream position, which is advanced), then families 1-3.
+ * Errors: B2M_ERR_MISSING_RNG without a usable rng, B2M_ERR_UNSUPPORTED on a multi-GPU context, B2M_ERR_INVALID_ARG for h /
+ * beta_h / neg_h at infinity or a neg key above D, B2M_ERR_SERIALIZATION for a G2 point off the twist. */
+int b2m_srs_check_powers(b2m_srs* srs, const uint8_t* h, const uint8_t* beta_h, size_t n_neg, const uint64_t* neg_keys,
+                         const uint8_t* neg_h, b2m_rng* rng, int* ok, int* bad_kind, size_t* bad_index);
 
 /* ---- Level 1: polynomial-commitment ABI --------------------------------------------------------- */
 

@@ -91,6 +91,9 @@ def lib():
         L.b2m_g1_to_uncompressed.argtypes = [vp, ci, vp, sz, vp]
         L.b2m_g1_decode_ark.argtypes = [vp, ci, vp, sz, ci, vp, P(sz), P(ci)]
         L.b2m_g2_decode_ark.argtypes = [vp, ci, vp, sz, ci, vp, P(sz), P(ci)]
+        L.b2m_g1_decode_lem.argtypes = [vp, ci, vp, sz, vp, P(sz), P(ci)]
+        L.b2m_g2_decode_lem.argtypes = [vp, ci, vp, sz, vp, P(sz), P(ci)]
+        L.b2m_srs_check_powers.argtypes = [vp, vp, vp, sz, vp, vp, vp, P(ci), P(ci), P(sz)]
         L.b2m_pairing_check.argtypes = [vp, ci, sz, vp, sz, vp, vp, vp, vp]
         L.b2m_g1_to_compressed.argtypes = [vp, ci, vp, sz, vp]
         L.b2m_g2_to_compressed.argtypes = [ci, vp, sz, vp]

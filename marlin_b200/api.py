@@ -18,6 +18,7 @@ import numpy as np
 from . import _lib, fields, srsfile
 
 PC_IDS = {"marlin_kzg10": _lib.PC_MARLIN_KZG10, "sonic_kzg10": _lib.PC_SONIC_KZG10}
+_CURVE_NAMES = {v: k for k, v in fields.CURVE_IDS.items()}
 
 
 class Context:
@@ -551,14 +552,101 @@ class Marlin:
         srs.g2 = (d["h"], d["beta_h"], d["neg_powers"])
         return srs
 
-    def load_ark_srs(self, path, compressed=True, degree_bounds=(), window_bits=0, window_tables=0):
+    def load_ptau(self, path, max_degree=None, check=True, rng=None, window_bits=0, window_tables=0):
+        """Load a snarkjs Powers-of-Tau file (marlin_b200/ptau.py) -- the output of a multi-party ceremony -- as a MarlinKZG10
+        SRS of max degree D = max_degree (default: the whole file, 2^(power+1) - 2).  powers_of_g = tauG1[0..=D], the gamma
+        powers {0, 1, 2} = alphaTauG1[0..=2] (alpha plays gamma: it is accumulated over the contributions like tau and known to
+        nobody if one contributor was honest), h = tauG2[0], beta_h = tauG2[1]; nothing else is read.  Every point is decoded
+        and validated on the GPU (coordinates below p, on the curve, in the prime-order subgroup) and must be finite; the first
+        bad one raises B2MError (B2M_ERR_SERIALIZATION) naming it, e.g. `tauG1[1048573]: not in the prime-order subgroup`.
+        check=True then decides on the GPU that the points are one chain of powers (b2m_srs_check_powers, with rng or an
+        OS-seeded ZkRng()); a break raises naming the point, e.g. `tauG1[7] is not tau times tauG1[6]`.  This proves the file
+        is a well-formed powers-of-tau SRS, not which ceremony made it.  SonicKZG10 is refused: the file has no
+        neg_powers_of_h.  verifier_key, save and save_ark work on the result as on any loaded SRS."""
+        from . import ptau
+        if self.pc == _lib.PC_SONIC_KZG10:
+            raise ValueError("a .ptau file holds no neg_powers_of_h: SonicKZG10 cannot use it (MarlinKZG10 can)")
+        f = ptau.read_ptau(path)
+        cid = self.curve_id
+        if f.curve_id != cid:
+            raise ValueError(f"{path} is a {_CURVE_NAMES[f.curve_id]} file, this Marlin instance is {_CURVE_NAMES[cid]}")
+        D = f.max_degree if max_degree is None else int(max_degree)
+        if D > f.max_degree:
+            raise ValueError(f"{path}: max degree {D} needs a power-{ptau.power_for_degree(D)} file; this one is power {f.power} "
+                             f"(max degree {f.max_degree})")
+        if D < 1:
+            raise ValueError(f"max degree {D} < 1")
+        if f.counts[4] < 3:
+            raise ValueError(f"{path}: alphaTauG1 holds {f.counts[4]} points, the SRS needs 3 (power >= 2)")
+        L = _lib.lib()
+        lq = _lib.LIMBS[cid][1]
+
+        def bad(field, i, reason):
+            raise _lib.B2MError(_lib.ERR_SERIALIZATION, f"{field}[{i}]: {reason}")
+
+        def g1(pts, field):
+            pts = np.ascontiguousarray(pts)
+            out = np.zeros((len(pts), 2 * lq), dtype=np.uint64)
+            bi, br = ctypes.c_size_t(0), ctypes.c_int(0)
+            rc = L.b2m_g1_decode_lem(self.ctx.handle, cid, _lib.ptr(pts.reshape(-1)), len(pts), _lib.ptr(out), ctypes.byref(bi), ctypes.byref(br))
+            if rc == _lib.ERR_SERIALIZATION:
+                bad(field, bi.value, _lib.POINT_REASONS.get(br.value, "invalid point"))
+            _lib.check(rc)
+            inf = np.flatnonzero(~out.any(axis=1))
+            if len(inf):
+                bad(field, int(inf[0]), "the point at infinity")
+            return out
+
+        powers = g1(f.tau_g1(D + 1), "tauG1")
+        gam = g1(f.alpha_tau_g1(3), "alphaTauG1")
+        g2in = np.ascontiguousarray(f.tau_g2(2))
+        g2 = np.zeros((2, 4 * f.n8), dtype=np.uint8)
+        bi, br = ctypes.c_size_t(0), ctypes.c_int(0)
+        rc = L.b2m_g2_decode_lem(self.ctx.handle, cid, _lib.ptr(g2in.reshape(-1)), 2, _lib.ptr(g2), ctypes.byref(bi), ctypes.byref(br))
+        if rc == _lib.ERR_SERIALIZATION:
+            bad("tauG2", bi.value, _lib.POINT_REASONS.get(br.value, "invalid point"))
+        _lib.check(rc)
+        for i in range(2):
+            if g2[i, -1] & 0x40:
+                bad("tauG2", i, "the point at infinity")
+        srs = self.srs_from_points(powers, gam, [0, 1, 2], window_bits, window_tables)
+        srs.g2 = (g2[0].tobytes(), g2[1].tobytes(), {})
+        if check:
+            names = {0: lambda i: f"tauG1[{i + 1}] is not tau times tauG1[{i}]" + (" (or tauG2[1] is not tau times tauG2[0])" if i == 0 else ""),
+                     1: lambda k: f"alphaTauG1[{k + 1}] is not tau times alphaTauG1[{k}]"}
+            self._check_powers(srs, g2[0], g2[1], [], None, rng, names)
+        return srs
+
+    def _check_powers(self, srs, h, beta_h, neg_keys, neg, rng, names):
+        """b2m_srs_check_powers; on a break the SRS is closed and B2MError (B2M_ERR_SERIALIZATION) raised with
+        names[family](index)"""
+        rng = rng if rng is not None else ZkRng()
+        ok, kind, idx = ctypes.c_int(0), ctypes.c_int(0), ctypes.c_size_t(0)
+        h, beta_h = np.ascontiguousarray(h, dtype=np.uint8), np.ascontiguousarray(beta_h, dtype=np.uint8)
+        keys = np.ascontiguousarray(neg_keys, dtype=np.uint64)
+        negb = np.ascontiguousarray(neg, dtype=np.uint8) if len(keys) else None
+        try:
+            _lib.check(_lib.lib().b2m_srs_check_powers(srs.handle, _lib.ptr(h), _lib.ptr(beta_h), len(keys), _lib.ptr(keys) if len(keys) else None,
+                                                       _lib.ptr(negb) if len(keys) else None, ctypes.byref(rng.c), ctypes.byref(ok),
+                                                       ctypes.byref(kind), ctypes.byref(idx)))
+        except Exception:
+            srs.close()
+            raise
+        if not ok.value:
+            srs.close()
+            raise _lib.B2MError(_lib.ERR_SERIALIZATION, names[kind.value](int(idx.value)))
+
+    def load_ark_srs(self, path, compressed=True, degree_bounds=(), window_bits=0, window_tables=0, check_powers=False, rng=None):
         """Load a raw arkworks `kzg10::UniversalParams` file, as `UniversalParams::serialize` (compressed=True) or
         `serialize_uncompressed` wrote it, with `deserialize` semantics: every point is decoded and validated on the GPU (flags,
         coordinates below p, on the curve, in the prime-order subgroup), and the first invalid one raises B2MError
         (B2M_ERR_SERIALIZATION) naming its field and index, e.g. `powers_of_g[1048573]: not in the prime-order subgroup`
         (BTreeMap fields are indexed by key).  The device key receives the gamma powers `universal_setup(degree_bounds=...)`
         would make -- indices 0, 1, 2 and D - d + {0, 1, 2} per bound d -- while the returned SRS keeps the whole file (every
-        gamma power, every G2 point, contiguous) for `verifier_key` and `save_ark`."""
+        gamma power, every G2 point, contiguous) for `verifier_key` and `save_ark`.  check_powers=True also decides on the GPU
+        that the points are one chain of powers of one beta (b2m_srs_check_powers over powers_of_g, the gamma powers on the
+        device and every neg_powers_of_h entry, with rng or an OS-seeded ZkRng()); a break raises B2MError naming the point,
+        e.g. `powers_of_g[7] is not beta times powers_of_g[6]`."""
         from . import srsfile
         L = _lib.lib()
         cid = self.curve_id
@@ -613,6 +701,12 @@ class Marlin:
         h, beta_h, neg = g2_out[0], g2_out[1], np.ascontiguousarray(g2_out[2:])
         srs.g2 = (h.tobytes(), beta_h.tobytes(), srsfile.G2Points(nkeys, neg))
         srs.ark = {"gamma_keys": gkeys, "gamma_limbs": gamma_all, "h": h, "beta_h": beta_h, "neg_keys": nkeys, "neg": neg}
+        if check_powers:
+            names = {0: lambda i: f"powers_of_g[{i + 1}] is not beta times powers_of_g[{i}]" + (" (or beta_h is not beta times h)" if i == 0 else ""),
+                     1: lambda k: f"powers_of_gamma_g[{k + 1}] is not beta times powers_of_gamma_g[{k}]",
+                     2: lambda k: f"neg_powers_of_h[{k}] is not beta^-{k} h (checked against powers_of_g[{k}])",
+                     3: lambda k: f"neg_powers_of_h[{k}] is not beta^-{k} h (or powers_of_gamma_g[{k}] is not beta^{k} gamma g)"}
+            self._check_powers(srs, h, beta_h, nkeys, neg, rng, names)
         return srs
 
     def srs_from_points(self, powers_limbs, gamma_limbs, gamma_indices, window_bits=0, window_tables=0):

@@ -1,5 +1,5 @@
 // Batch conversion of ark-serialize G1 / G2 points and Fr elements on the GPU (the SRS and index-key loaders:
-// b2m_g1_decode_ark, b2m_g2_decode_ark, b2m_g1_to_compressed, b2m_fr_decode_ark, b2m_fr_to_canonical).  Definitions in ark_points_impl.cuh, instantiated per curve by inst_ark_{bls,bn,bls377}.cu.
+// b2m_g1_decode_ark, b2m_g2_decode_ark, b2m_g1_decode_lem, b2m_g2_decode_lem, b2m_g1_to_compressed, b2m_fr_decode_ark, b2m_fr_to_canonical).  Definitions in ark_points_impl.cuh, instantiated per curve by inst_ark_{bls,bn,bls377}.cu.
 #pragma once
 #include "common.cuh"
 #include "field.cuh"
@@ -22,6 +22,12 @@ ArkBad g1_decode_ark(Ctx& cx, const uint8_t* bytes, size_t n, bool compressed, u
 // n points in either form -> uncompressed canonical bytes (4 * sizeof(Fq) each).
 template <class Fq>
 ArkBad g2_decode_ark(Ctx& cx, const uint8_t* bytes, size_t n, bool compressed, uint8_t* out);
+// n snarkjs LEM points (.ptau files; g1_decode.cuh) -> affine Montgomery limbs / uncompressed canonical ark bytes, with the
+// same chunking and stopping rule as the ark forms.
+template <class Fq>
+ArkBad g1_decode_lem_points(Ctx& cx, const uint8_t* bytes, size_t n, uint64_t* out_xy);
+template <class Fq>
+ArkBad g2_decode_lem_points(Ctx& cx, const uint8_t* bytes, size_t n, uint8_t* out);
 // affine Montgomery limbs -> compressed bytes (sizeof(Fq) each).
 template <class Fq>
 void g1_to_compressed(Ctx& cx, const uint64_t* points_xy, size_t n, uint8_t* out);

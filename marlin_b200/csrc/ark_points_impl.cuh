@@ -33,6 +33,27 @@ __global__ void g2_decode_ark_kernel(const uint8_t* bytes, size_t n, uint8_t* ou
   if (s != G1_OK) atomicMin(first_bad, (unsigned long long)i);
 }
 
+// snarkjs LEM points (.ptau files): a form of their own, so the ark kernels above keep their register allocation
+template <class Fq>
+__global__ void g1_decode_lem_kernel(const uint8_t* bytes, size_t n, Affine<Fq>* out, int* status, unsigned long long* first_bad) {
+  const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  Affine<Fq> p;
+  const int s = g1_decode_lem<Fq>(bytes + i * (Fq::N * 8), &p);
+  out[i] = p;
+  status[i] = s;
+  if (s != G1_OK) atomicMin(first_bad, (unsigned long long)i);
+}
+
+template <class Fq>
+__global__ void g2_decode_lem_kernel(const uint8_t* bytes, size_t n, uint8_t* out, int* status, unsigned long long* first_bad) {
+  const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int s = g2_decode_lem<Fq>(bytes + i * (Fq::N * 16), out + i * (Fq::N * 16));
+  status[i] = s;
+  if (s != G1_OK) atomicMin(first_bad, (unsigned long long)i);
+}
+
 template <class Fq>
 __global__ void g1_compress_kernel(const Affine<Fq>* in, size_t n, uint8_t* out) {
   const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
@@ -90,6 +111,22 @@ ArkBad g2_decode_ark(Ctx& cx, const uint8_t* bytes, size_t n, bool compressed, u
                            [&](const uint8_t* din, size_t m, uint8_t* dout, int* st, unsigned long long* bad) {
                              if (compressed) g2_decode_ark_kernel<Fq, true><<<div_up(m, 128), 128, 0, cx.stream>>>(din, m, dout, st, bad);
                              else g2_decode_ark_kernel<Fq, false><<<div_up(m, 128), 128, 0, cx.stream>>>(din, m, dout, st, bad);
+                           });
+}
+
+template <class Fq>
+ArkBad g1_decode_lem_points(Ctx& cx, const uint8_t* bytes, size_t n, uint64_t* out_xy) {
+  return ark_decode_chunks(cx, bytes, n, Fq::N * 8, reinterpret_cast<uint8_t*>(out_xy), sizeof(Affine<Fq>), "lem_g1_decode",
+                           [&](const uint8_t* din, size_t m, uint8_t* dout, int* st, unsigned long long* bad) {
+                             g1_decode_lem_kernel<Fq><<<div_up(m, 128), 128, 0, cx.stream>>>(din, m, reinterpret_cast<Affine<Fq>*>(dout), st, bad);
+                           });
+}
+
+template <class Fq>
+ArkBad g2_decode_lem_points(Ctx& cx, const uint8_t* bytes, size_t n, uint8_t* out) {
+  return ark_decode_chunks(cx, bytes, n, Fq::N * 16, out, Fq::N * 16, "lem_g2_decode",
+                           [&](const uint8_t* din, size_t m, uint8_t* dout, int* st, unsigned long long* bad) {
+                             g2_decode_lem_kernel<Fq><<<div_up(m, 128), 128, 0, cx.stream>>>(din, m, dout, st, bad);
                            });
 }
 
@@ -180,6 +217,8 @@ void fr_to_canonical(Ctx& cx, const Fr* in_dev, size_t n, uint8_t* out) {
 #define B2M_INSTANTIATE_ARK_POINTS(FQ)                                                                  \
   template ArkBad g1_decode_ark<FQ>(Ctx&, const uint8_t*, size_t, bool, uint64_t*);                  \
   template ArkBad g2_decode_ark<FQ>(Ctx&, const uint8_t*, size_t, bool, uint8_t*);                   \
+  template ArkBad g1_decode_lem_points<FQ>(Ctx&, const uint8_t*, size_t, uint64_t*);                         \
+  template ArkBad g2_decode_lem_points<FQ>(Ctx&, const uint8_t*, size_t, uint8_t*);                          \
   template void g1_to_compressed<FQ>(Ctx&, const uint64_t*, size_t, uint8_t*);
 #define B2M_INSTANTIATE_ARK_FR(FR)                                                                      \
   template ArkBad fr_decode_ark<FR>(Ctx&, const uint8_t*, size_t, FR*);                              \

@@ -280,6 +280,30 @@ int b2m_g2_decode_ark(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, i
       throw Error(B2M_ERR_SERIALIZATION, fmt("G2 point %zu: %s", bad.index, point_status_name(bad.reason)));
   });
 }
+int b2m_g1_decode_lem(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, uint64_t* out_xy, size_t* bad_index, int* bad_reason) {
+  return guard([&] {
+    B2M_REQUIRE(ctx && ((bytes && out_xy) || n == 0), B2M_ERR_INVALID_ARG, "null argument");
+    require_curve(curve);
+    ctx->cx.use();
+    const ArkBad bad = n == 0 ? ArkBad{0, G1_OK} : with_curve(curve, [&](auto t) {
+      return g1_decode_lem_points<typename decltype(t)::Fq>(ctx->cx, bytes, n, out_xy);
+    });
+    if (ark_fail(bad, bad_index, bad_reason) != B2M_OK)
+      throw Error(B2M_ERR_SERIALIZATION, fmt("G1 point %zu: %s", bad.index, point_status_name(bad.reason)));
+  });
+}
+int b2m_g2_decode_lem(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t n, uint8_t* out_uncompressed, size_t* bad_index, int* bad_reason) {
+  return guard([&] {
+    B2M_REQUIRE(ctx && ((bytes && out_uncompressed) || n == 0), B2M_ERR_INVALID_ARG, "null argument");
+    require_curve(curve);
+    ctx->cx.use();
+    const ArkBad bad = n == 0 ? ArkBad{0, G1_OK} : with_curve(curve, [&](auto t) {
+      return g2_decode_lem_points<typename decltype(t)::Fq>(ctx->cx, bytes, n, out_uncompressed);
+    });
+    if (ark_fail(bad, bad_index, bad_reason) != B2M_OK)
+      throw Error(B2M_ERR_SERIALIZATION, fmt("G2 point %zu: %s", bad.index, point_status_name(bad.reason)));
+  });
+}
 int b2m_pairing_check(b2m_ctx* ctx, int curve, size_t n_g2, const uint8_t* g2, size_t n_products, const size_t* product_off,
                       const uint64_t* g1_xy, const uint32_t* g2_index, int* verdicts) {
   return guard([&] {
@@ -812,6 +836,20 @@ int b2m_verify_multi(size_t n_keys, b2m_vk* const* vks, size_t n, const uint32_t
     for (size_t k = 0; k < n_keys; k++) impls[k] = vks[k]->impl.get();
     vks[0]->ctx->cx.use();
     impls[0]->verify_multi(n_keys, impls.data(), n, key_of, public_inputs, n_inputs, proofs, proof_lens, rng, verdicts);
+  });
+}
+
+int b2m_srs_check_powers(b2m_srs* srs, const uint8_t* h, const uint8_t* beta_h, size_t n_neg, const uint64_t* neg_keys, const uint8_t* neg_h,
+                         b2m_rng* rng, int* ok, int* bad_kind, size_t* bad_index) {
+  return guard([&] {
+    B2M_REQUIRE(srs && h && beta_h && ok && (n_neg == 0 || (neg_keys && neg_h)), B2M_ERR_INVALID_ARG, "null argument");
+    B2M_REQUIRE(srs->ctx->cx.world <= 1, B2M_ERR_UNSUPPORTED, "the power check on a multi-GPU context");
+    require_verify_rng(rng);
+    *ok = 0;
+    srs->ctx->cx.use();
+    with_curve(srs->curve, [&](auto t) {
+      srs_check_powers<typename decltype(t)::Fr, typename decltype(t)::Fq>(srs, h, beta_h, n_neg, neg_keys, neg_h, rng, ok, bad_kind, bad_index);
+    });
   });
 }
 

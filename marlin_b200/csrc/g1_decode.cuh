@@ -147,6 +147,15 @@ B2M_HD int g1_decompress(const uint8_t* bytes, Affine<Fq>* out) {
   return G1_OK;
 }
 
+// the shared tail of the uncompressed forms: the curve equation and the subgroup; *out = p when both hold
+template <class Fq>
+B2M_HD int g1_check_store(const Affine<Fq>& p, Affine<Fq>* out) {
+  if (p.y.sqr() != p.x.sqr() * p.x + Fq::from_u64(G1Curve<Fq>::b)) return G1_NOT_ON_CURVE;
+  if (!g1_in_subgroup(p)) return G1_NOT_IN_SUBGROUP;
+  *out = p;
+  return G1_OK;
+}
+
 // `deserialize_uncompressed` (checked): x || y, flags in y's last byte.  The infinity flag accepts any canonical coordinates,
 // as ark-serialize does; the sign bit carries no meaning in this form.
 template <class Fq>
@@ -161,11 +170,21 @@ B2M_HD int g1_decode_uncompressed(const uint8_t* bytes, Affine<Fq>* out) {
   if (!fq_below_modulus(x)) return G1_X_NOT_CANONICAL;
   if (!fq_below_modulus(y)) return G1_Y_NOT_CANONICAL;
   if (flags & 1u) return G1_OK;  // infinity
-  const Affine<Fq> p{Fq::from_canonical(x), Fq::from_canonical(y)};
-  if (p.y.sqr() != p.x.sqr() * p.x + Fq::from_u64(G1Curve<Fq>::b)) return G1_NOT_ON_CURVE;
-  if (!g1_in_subgroup(p)) return G1_NOT_IN_SUBGROUP;
-  *out = p;
-  return G1_OK;
+  return g1_check_store(Affine<Fq>{Fq::from_canonical(x), Fq::from_canonical(y)}, out);
+}
+
+// snarkjs "LEM" form (.ptau files): x || y, each little-endian MONTGOMERY limbs with R = 2^(64 * limbs) -- for these fields
+// exactly the device's 32-bit-limb Montgomery form, so no conversion.  No flags: all-zero bytes are the point at infinity
+// [U snarkjs].  A limb vector >= p is not a field element (a non-reduced representative) and is rejected.
+template <class Fq>
+B2M_HD int g1_decode_lem(const uint8_t* bytes, Affine<Fq>* out) {
+  constexpr int N = Fq::N;
+  const Fq x = fq_load<Fq>(bytes), y = fq_load<Fq>(bytes + N * 4);
+  *out = Affine<Fq>::inf();
+  if (x.is_zero() && y.is_zero()) return G1_OK;  // infinity ((0, 0) is on none of the curves: b != 0)
+  if (!fq_below_modulus(x)) return G1_X_NOT_CANONICAL;
+  if (!fq_below_modulus(y)) return G1_Y_NOT_CANONICAL;
+  return g1_check_store(Affine<Fq>{x, y}, out);
 }
 
 // affine Montgomery -> `serialize` (compressed) bytes: canonical x, bit 7 = y is the larger root, infinity = zero + bit 6

@@ -73,6 +73,24 @@ B2M_HD int g2_decode(const uint8_t* bytes, bool compressed, uint8_t* out) {
   return G1_OK;
 }
 
+// snarkjs "LEM" form: x.c0 || x.c1 || y.c0 || y.c1, each little-endian Montgomery limbs (g1_decode_lem); all-zero bytes are
+// infinity.  -> uncompressed canonical bytes as g2_decode writes them
+template <class Fq>
+B2M_HD int g2_decode_lem(const uint8_t* bytes, uint8_t* out) {
+  constexpr int NB = Fq::N * 4;
+  const Fq x0 = fq_load<Fq>(bytes), x1 = fq_load<Fq>(bytes + NB), y0 = fq_load<Fq>(bytes + 2 * NB), y1 = fq_load<Fq>(bytes + 3 * NB);
+  const Fq2<Fq> zero = Fq2<Fq>::zero();
+  g2_store_uncompressed<Fq>(zero, zero, true, out);
+  if (x0.is_zero() && x1.is_zero() && y0.is_zero() && y1.is_zero()) return G1_OK;  // infinity
+  if (!fq_below_modulus(x0) || !fq_below_modulus(x1)) return G1_X_NOT_CANONICAL;
+  if (!fq_below_modulus(y0) || !fq_below_modulus(y1)) return G1_Y_NOT_CANONICAL;
+  const Fq2<Fq> x{x0, x1}, y{y0, y1};
+  if (y.sqr() != x.sqr() * x + G2Curve<Fq>::b()) return G1_NOT_ON_CURVE;
+  if (!g2_in_subgroup(x, y)) return G1_NOT_IN_SUBGROUP;
+  g2_store_uncompressed<Fq>(x, y, false, out);
+  return G1_OK;
+}
+
 // uncompressed canonical bytes (as g2_decode writes them) -> compressed bytes; no field multiplication needed
 template <class Fq>
 B2M_HD void g2_compress(const uint8_t* in, uint8_t* out) {

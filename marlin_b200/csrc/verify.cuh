@@ -5,6 +5,8 @@
 
 #include "common.cuh"
 
+struct b2m_srs;
+
 namespace b2m {
 
 struct VerifierBase {
@@ -40,6 +42,11 @@ struct VkArgs {
 template <class Fq>
 void pairing_check(Ctx& cx, size_t n_g2, const uint8_t* g2, size_t n_products, const size_t* off, const uint64_t* g1_xy, const uint32_t* g2_index,
                    int* verdicts);
+
+// b2m_srs_check_powers for one curve (srs_check_impl.cuh; instantiated with the verifier of that curve)
+template <class Fr, class Fq>
+void srs_check_powers(b2m_srs* srs, const uint8_t* h, const uint8_t* beta_h, size_t n_neg, const uint64_t* neg_keys, const uint8_t* neg_h,
+                      b2m_rng* rng, int* ok, int* bad_kind, size_t* bad_index);
 
 VerifierBase* make_verifier_bls(Ctx& cx, const VkArgs& a);
 VerifierBase* make_verifier_bn(Ctx& cx, const VkArgs& a);
