@@ -132,6 +132,13 @@ extern "C" {
     pub fn b2m_fr_decode_ark(ctx: *mut b2m_ctx, curve: c_int, bytes: *const u8, n: usize, out_limbs: *mut u64, bad_index: *mut usize) -> c_int;
     pub fn b2m_fr_to_canonical(ctx: *mut b2m_ctx, curve: c_int, limbs: *const u64, n: usize, out: *mut u8) -> c_int;
     pub fn b2m_domain_ark(curve: c_int, log_size: c_uint, out: *mut u8) -> c_int;
+    pub fn b2m_circom_constraint_rows(bytes: *const u8, len: usize, m: usize, row_ptr_a: *mut u64, row_ptr_b: *mut u64, row_ptr_c: *mut u64,
+                                      end: *mut usize, bad_constraint: *mut usize, bad_reason: *mut c_int) -> c_int;
+    pub fn b2m_circom_decode_constraints(ctx: *mut b2m_ctx, curve: c_int, bytes: *const u8, len: usize, m: usize, row_ptrs: *const *const u64,
+                                         n_wires: u64, ni0: u64, shift: u64, out_row_ptr: *const *mut u64, out_col: *const *mut u64,
+                                         out_coeff: *const *mut u64, bad_matrix: *mut c_int, bad_term: *mut usize, bad_reason: *mut c_int) -> c_int;
+    pub fn b2m_r1cs_check(ctx: *mut b2m_ctx, curve: c_int, nc: usize, nv: usize, ni: usize, a: *const b2m_matrix, b: *const b2m_matrix,
+                          c: *const b2m_matrix, instance: *const u64, witness: *const u64, bad_row: *mut usize) -> c_int;
     pub fn b2m_ark_matrix_rows(bytes: *const u8, len: usize, n_rows: usize, entry_bytes: usize, row_ptr: *mut u64, end: *mut usize,
                                bad_row: *mut usize, bad_reason: *mut c_int) -> c_int;
     pub fn b2m_prove(idx: *mut b2m_index, formatted_input: *const u64, n_input: usize, witness: *const u64, n_witness: usize,

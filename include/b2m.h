@@ -226,6 +226,33 @@ int b2m_domain_ark(int curve, unsigned log_size, uint8_t* out);
 int b2m_ark_matrix_rows(const uint8_t* bytes, size_t len, size_t n_rows, size_t entry_bytes, uint64_t* row_ptr, size_t* end,
                         size_t* bad_row, int* bad_reason);
 
+/* circom `.r1cs` files [U circom r1csfile]: section 2 holds m constraints, each three linear combinations A, B, C, each a
+ * u32 term count followed by that many (u32 wire, 32-byte canonical little-endian coefficient) terms (n8 = 32).
+ *
+ * b2m_circom_constraint_rows walks the term counts once on the host (no context) and writes the three term-count prefix
+ * sums row_ptr_{a,b,c}[0..=m].  LC j of constraint k then starts at byte 4 (3k + j) + 36 (terms before it).  *end receives
+ * the bytes the m constraints take (a caller compares it with the section size).  A count truncated by len
+ * (*bad_reason = 1) or terms running past len (2) fail with B2M_ERR_SERIALIZATION; *bad_constraint receives the
+ * constraint and b2m_last_error() names it and its matrix, e.g. "constraints[12].B: truncated in the term count".
+ *
+ * b2m_circom_decode_constraints decodes the section on the GPU, in chunks of whole constraints (device scratch stays
+ * bounded): wire w goes to column w when w < ni0 (= 1 + nPubOut + nPubIn) and to w + shift otherwise (the instance padding
+ * of Marlin's indexer), coefficients to Montgomery form, and every row to normal form: columns ascending, equal columns
+ * summed mod r, zero sums dropped.  out_row_ptr[j] receives m + 1 entries; out_col[j] / out_coeff[j] (4 u64 limbs each)
+ * must hold row_ptrs[j][m] entries, as normalising never adds one; matrix j ends with out_row_ptr[j][m] entries.  A wire
+ * >= n_wires (*bad_reason = 1) or a coefficient not below r (2) fails with B2M_ERR_SERIALIZATION; *bad_matrix (0/1/2 =
+ * A/B/C) and *bad_term (index into that matrix's terms, row_ptrs[j]) name the lowest such term in file order.
+ *
+ * b2m_r1cs_check is ark-relations' `which_is_unsatisfied` for any padded R1CS (the b2m_index_create form, with the
+ * formatted instance and the witness as b2m_prove takes them): *bad_row receives the lowest row r with
+ * <A_r, z> * <B_r, z> != <C_r, z>, or nc when every row holds.  A column >= nv fails with B2M_ERR_INVALID_ARG.  The prover
+ * does not call it: as in the reference, proving an unsatisfied instance is not refused. */
+int b2m_circom_constraint_rows(const uint8_t* bytes, size_t len, size_t m, uint64_t* row_ptr_a, uint64_t* row_ptr_b, uint64_t* row_ptr_c,
+                               size_t* end, size_t* bad_constraint, int* bad_reason);
+int b2m_circom_decode_constraints(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t len, size_t m, const uint64_t* const* row_ptrs,
+                                  uint64_t n_wires, uint64_t ni0, uint64_t shift, uint64_t* const* out_row_ptr, uint64_t* const* out_col,
+                                  uint64_t* const* out_coeff, int* bad_matrix, size_t* bad_term, int* bad_reason);
+
 /* The caller's `zk_rng: &mut R` / `rng: Option<&mut dyn RngCore>` (reference src/lib.rs:154,125).  Two forms:
  *  - kind = B2M_RNG_CHACHA8/12/20, the fast path for the generators the reference's tests and benches use
  *    (`ark_std::test_rng()` = ChaCha12, `rand_chacha::ChaChaRng` = ChaCha20): the stream is described by its key and
@@ -340,6 +367,10 @@ typedef struct {
   const uint64_t* col;     /* nnz column (variable) indices */
   const uint64_t* coeff;   /* nnz * 4 limbs */
 } b2m_matrix;
+
+/* (b2m_r1cs_check: see the circom section above) */
+int b2m_r1cs_check(b2m_ctx* ctx, int curve, size_t nc, size_t nv, size_t ni, const b2m_matrix* a, const b2m_matrix* b, const b2m_matrix* c,
+                   const uint64_t* instance, const uint64_t* witness, size_t* bad_row);
 
 /* Replaces `Marlin::index` (reference src/lib.rs:100-148): AHP indexer
  * (src/ahp/indexer.rs:151-234, src/ahp/constraint_systems.rs:125-262) + `PC::trim` +

@@ -101,6 +101,8 @@ def lib():
         L.b2m_fr_to_canonical.argtypes = [vp, ci, vp, sz, vp]
         L.b2m_domain_ark.argtypes = [ci, ctypes.c_uint, vp]
         L.b2m_ark_matrix_rows.argtypes = [vp, sz, sz, sz, vp, P(sz), P(sz), P(ci)]
+        L.b2m_circom_constraint_rows.argtypes = [vp, sz, sz, vp, vp, vp, P(sz), P(sz), P(ci)]
+        L.b2m_circom_decode_constraints.argtypes = [vp, ci, vp, sz, sz, vp, u64, u64, u64, vp, vp, vp, P(ci), P(sz), P(ci)]
         L.b2m_pc_commit.argtypes = [vp, ci, sz, vp, vp, vp, vp, P(Rng), vp, vp, vp, vp, sz]
         L.b2m_pc_open.argtypes = [vp, ci, sz, vp, vp, vp, vp, vp, sz, ctypes.c_int64, vp, vp, vp, P(ci), vp]
         L.b2m_trim.argtypes = [vp, ci, sz, sz, vp, sz, P(vp)]
@@ -113,6 +115,7 @@ def lib():
         L.b2m_ck_open_combinations.argtypes = [vp, sz, vp, vp, vp, vp, vp, vp, sz, sz, vp, vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, vp]
         if hasattr(L, "b2m_index_create"):
             L.b2m_index_create.argtypes = [vp, ci, sz, sz, sz, P(Matrix), P(Matrix), P(Matrix), P(vp)]
+            L.b2m_r1cs_check.argtypes = [vp, ci, sz, sz, sz, P(Matrix), P(Matrix), P(Matrix), vp, vp, P(sz)]
             L.b2m_index_destroy.argtypes = [vp]
             L.b2m_index_destroy.restype = None
             L.b2m_index_vk_bytes.argtypes = [vp, vp, sz, P(sz)]

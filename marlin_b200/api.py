@@ -824,6 +824,105 @@ class Marlin:
                                       ctypes.byref(a), ctypes.byref(b), ctypes.byref(c), ctypes.byref(h)))
         return IndexProverKey(srs, h, r1cs, self.pc)
 
+    # -- circom circuits (marlin_b200/circom.py) ---------------------------------------------------------
+    def load_r1cs(self, path):
+        """The matrices of a circom `.r1cs` file as the padded, squared R1CS `Marlin::index` takes (instance and witness None;
+        enough for `index`, `IndexProverKey.save` and `verifier_key`).  Wires 1 .. nPubOut + nPubIn are the public inputs, in
+        snarkjs `public.json` order; wire w goes to column w (w < 1 + nPubOut + nPubIn) or past the instance padding, as
+        ark-circom and the indexer place it (r1cs.Shape), and circom constraint k is row k.  The constraint section is
+        decoded on the GPU, every row in normal form (columns ascending, equal wires summed, zero sums dropped).  A bad term
+        raises naming it, e.g. `constraints[12].B[3]: wire 4097 >= nWires 4096`."""
+        from . import circom
+        from . import r1cs as gr1cs
+        L = _lib.lib()
+        cid = self.curve_id
+        f = circom.read_r1cs(path)
+        circom.check_prime(path, "section 1 (header)", f.prime, cid)
+        sh = gr1cs.Shape(f.ni0, f.n_wires - f.ni0, f.m)
+        rps = circom.constraint_rows(f)
+        nnz = [int(r[-1]) for r in rps]
+        out_rp = [np.zeros(f.m + 1, dtype=np.uint64) for _ in range(3)]
+        cols = [np.zeros(max(n, 1), dtype=np.uint64) for n in nnz]
+        coeffs = [np.zeros((max(n, 1), 4), dtype=np.uint64) for n in nnz]
+        arr = lambda xs: (ctypes.c_void_p * 3)(*[x.ctypes.data for x in xs])  # noqa: E731
+        bm, bt, br = ctypes.c_int(0), ctypes.c_size_t(0), ctypes.c_int(0)
+        data = f.constraints
+        rc = L.b2m_circom_decode_constraints(self.ctx.handle, cid, data.ctypes.data if len(data) else None, len(data), f.m, arr(rps), f.n_wires,
+                                             f.ni0, sh.shift, arr(out_rp), arr(cols), arr(coeffs), ctypes.byref(bm), ctypes.byref(bt),
+                                             ctypes.byref(br))
+        if rc == _lib.ERR_SERIALIZATION:
+            j, t = bm.value, bt.value
+            k = int(np.searchsorted(rps[j], np.uint64(t), side="right")) - 1
+            i = t - int(rps[j][k])
+            at = f"constraints[{k}].{circom.MATRICES[j]}[{i}]"
+            if br.value == 1:
+                off = circom.term_offset(rps, k, j, i)
+                wire = int.from_bytes(bytes(data[off:off + 4]), "little")
+                raise _lib.B2MError(rc, f"{at}: wire {wire} >= nWires {f.n_wires}")
+            raise _lib.B2MError(rc, f"{at}: coefficient not below r")
+        _lib.check(rc)
+        mats = []
+        for j in range(3):
+            n = int(out_rp[j][-1])
+            row_ptr = np.concatenate([out_rp[j], np.full(sh.pad_rows, n, dtype=np.uint64)])
+            if n == 0:  # the placeholder `from_rows` emits for an empty matrix
+                mats.append((row_ptr, np.zeros(1, dtype=np.uint64), np.zeros((1, 4), dtype=np.uint64)))
+            else:
+                mats.append((row_ptr, cols[j][:n], coeffs[j][:n]))
+        out = gr1cs.R1CS(cid, sh.ni, mats[0], mats[1], mats[2], None, None, num_variables=sh.size)
+        out.circom = f.info()
+        return out
+
+    def load_wtns(self, r1cs, path, check=True):
+        """`r1cs` (from load_r1cs) with the assignment of a circom `.wtns` file: instance = wires 0 .. nPubOut + nPubIn
+        padded with zeros, witness = the remaining wires then ones for the squaring.  Values are decoded and checked below r
+        on the GPU; wire 0 must be one.  check=True runs `which_is_unsatisfied` and raises naming the lowest failing
+        constraint, e.g. `constraint 1234 is not satisfied`."""
+        from . import circom
+        from . import r1cs as gr1cs
+        info = r1cs.circom
+        if info is None:
+            raise ValueError("load_wtns takes an R1CS from load_r1cs")
+        L = _lib.lib()
+        cid = self.curve_id
+        f = circom.read_wtns(path)
+        circom.check_prime(path, "section 1 (header)", f.prime, cid)
+        if f.n_witness != info.n_wires:
+            raise ValueError(f"{path}: section 1 (header): nWitness = {f.n_witness}, the circuit has nWires = {info.n_wires}")
+        vals = np.zeros((f.n_witness, 4), dtype=np.uint64)
+        bi = ctypes.c_size_t(0)
+        rc = L.b2m_fr_decode_ark(self.ctx.handle, cid, f.values.ctypes.data, f.n_witness, _lib.ptr(vals), ctypes.byref(bi))
+        if rc == _lib.ERR_SERIALIZATION:
+            raise _lib.B2MError(rc, f"witness[{bi.value}]: not below r")
+        _lib.check(rc)
+        one = _lib.ints_to_limbs([fields.fr_to_mont(cid, 1)], 4)[0]
+        if not np.array_equal(vals[0], one):
+            raise ValueError(f"{path}: witness[0] is {fields.fr_from_mont(cid, _lib.limbs_to_ints(vals[0])[0])}, wire 0 is the constant one")
+        ni0 = 1 + info.n_pub_out + info.n_pub_in
+        sh = gr1cs.Shape(ni0, info.n_wires - ni0, info.m_constraints)
+        inst = np.concatenate([vals[:ni0], np.zeros((sh.shift, 4), dtype=np.uint64)])
+        wit = np.concatenate([vals[ni0:], np.tile(one, (sh.pad_witness, 1))])
+        out = gr1cs.R1CS(cid, sh.ni, r1cs.a, r1cs.b, r1cs.c, inst, wit)
+        out.circom = info
+        if check:
+            bad = self.which_is_unsatisfied(out)
+            if bad is not None:
+                raise ValueError(f"{path}: constraint {bad} is not satisfied")
+        return out
+
+    def which_is_unsatisfied(self, r1cs):
+        """ark-relations' `which_is_unsatisfied` on the GPU (b2m_r1cs_check): the lowest row r of the padded instance with
+        <A_r, z> * <B_r, z> != <C_r, z>, or None when every row holds.  Circom constraint k is row k."""
+        if r1cs.witness is None:
+            raise ValueError("the instance has no assignment (load_wtns gives one)")
+        a, b, c = r1cs.matrices()
+        inst, wit = np.ascontiguousarray(r1cs.instance), np.ascontiguousarray(r1cs.witness)
+        bad = ctypes.c_size_t(0)
+        _lib.check(_lib.lib().b2m_r1cs_check(self.ctx.handle, self.curve_id, r1cs.num_constraints, r1cs.num_variables, r1cs.num_instance,
+                                             ctypes.byref(a), ctypes.byref(b), ctypes.byref(c), _lib.ptr(inst),
+                                             _lib.ptr(wit) if len(wit) else None, ctypes.byref(bad)))
+        return None if bad.value == r1cs.num_constraints else bad.value
+
     # -- index key files (marlin_b200/keyfile.py) --------------------------------------------------------
     def _decode_g1(self, pts, field, compressed, names=int):
         """ark-serialize G1 bytes (n, size) -> affine limbs, validated on the GPU; an invalid point raises naming field[index]"""

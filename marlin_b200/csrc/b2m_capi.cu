@@ -8,6 +8,7 @@
 #include "g2_host.hpp"
 #include "ark_points.cuh"
 #include "g2_decode.cuh"
+#include "circom.cuh"
 
 namespace b2m {
 thread_local std::string g_last_error;
@@ -399,6 +400,72 @@ int b2m_ark_matrix_rows(const uint8_t* bytes, size_t len, size_t n_rows, size_t 
       pos += 8 + n * entry_bytes;
     }
     *end = pos;
+  });
+}
+
+// The term-count chain of a circom `.r1cs` constraint section (host; one step per linear combination, nothing else can be
+// done in parallel).  Entries are (u32 wire, 32-byte coefficient): n8 = 32.
+int b2m_circom_constraint_rows(const uint8_t* bytes, size_t len, size_t m, uint64_t* row_ptr_a, uint64_t* row_ptr_b, uint64_t* row_ptr_c,
+                               size_t* end, size_t* bad_constraint, int* bad_reason) {
+  if (end) *end = 0;
+  if (bad_constraint) *bad_constraint = 0;
+  if (bad_reason) *bad_reason = 0;
+  return guard([&] {
+    B2M_REQUIRE(row_ptr_a && row_ptr_b && row_ptr_c && end && (bytes || len == 0), B2M_ERR_INVALID_ARG, "null argument");
+    uint64_t* rp[3] = {row_ptr_a, row_ptr_b, row_ptr_c};
+    size_t pos = 0;
+    for (int j = 0; j < 3; j++) rp[j][0] = 0;
+    for (size_t k = 0; k < m; k++) {
+      for (int j = 0; j < 3; j++) {
+        auto fail = [&](int reason, const std::string& what) {
+          *end = pos;
+          if (bad_constraint) *bad_constraint = k;
+          if (bad_reason) *bad_reason = reason;
+          throw Error(B2M_ERR_SERIALIZATION, fmt("constraints[%zu].%c: %s", k, "ABC"[j], what.c_str()));
+        };
+        if (len - pos < 4) fail(1, "truncated in the term count");
+        uint32_t n = 0;
+        memcpy(&n, bytes + pos, 4);
+        if (n > (len - pos - 4) / CIRCOM_TERM_BYTES) fail(2, fmt("%u terms run past the end of the section", n));
+        rp[j][k + 1] = rp[j][k] + n;
+        pos += 4 + (size_t)n * CIRCOM_TERM_BYTES;
+      }
+    }
+    *end = pos;
+  });
+}
+int b2m_circom_decode_constraints(b2m_ctx* ctx, int curve, const uint8_t* bytes, size_t len, size_t m, const uint64_t* const* row_ptrs,
+                                  uint64_t n_wires, uint64_t ni0, uint64_t shift, uint64_t* const* out_row_ptr, uint64_t* const* out_col,
+                                  uint64_t* const* out_coeff, int* bad_matrix, size_t* bad_term, int* bad_reason) {
+  if (bad_matrix) *bad_matrix = 0;
+  if (bad_term) *bad_term = 0;
+  if (bad_reason) *bad_reason = 0;
+  return guard([&] {
+    B2M_REQUIRE(ctx && row_ptrs && out_row_ptr && out_col && out_coeff && (bytes || len == 0), B2M_ERR_INVALID_ARG, "null argument");
+    for (int j = 0; j < 3; j++)
+      B2M_REQUIRE(row_ptrs[j] && out_row_ptr[j] && ((out_col[j] && out_coeff[j]) || row_ptrs[j][m] == 0), B2M_ERR_INVALID_ARG, "null argument");
+    require_curve(curve);
+    ctx->cx.use();
+    const CircomBad bad = with_curve(curve, [&](auto t) {
+      return circom_decode_constraints<typename decltype(t)::Fr>(ctx->cx, bytes, len, m, row_ptrs, n_wires, ni0, shift, out_row_ptr, out_col, out_coeff);
+    });
+    if (bad.reason) {
+      if (bad_matrix) *bad_matrix = bad.matrix;
+      if (bad_term) *bad_term = bad.term;
+      if (bad_reason) *bad_reason = bad.reason;
+      throw Error(B2M_ERR_SERIALIZATION, fmt("matrix %c term %zu: %s", "ABC"[bad.matrix], bad.term,
+                                             bad.reason == 1 ? "wire >= nWires" : "coefficient not below r"));
+    }
+  });
+}
+int b2m_r1cs_check(b2m_ctx* ctx, int curve, size_t nc, size_t nv, size_t ni, const b2m_matrix* a, const b2m_matrix* b, const b2m_matrix* c,
+                   const uint64_t* instance, const uint64_t* witness, size_t* bad_row) {
+  return guard([&] {
+    B2M_REQUIRE(ctx && a && b && c && instance && bad_row && (witness || nv == ni), B2M_ERR_INVALID_ARG, "null argument");
+    require_curve(curve);
+    ctx->cx.use();
+    const b2m_matrix* mats[3] = {a, b, c};
+    *bad_row = with_curve(curve, [&](auto t) { return r1cs_check<typename decltype(t)::Fr>(ctx->cx, nc, nv, ni, mats, instance, witness); });
   });
 }
 

@@ -21,14 +21,16 @@ def _next_pow2(n):
 class R1CS:
     """Padded, squared instance: matrices as CSR numpy arrays, assignments as Montgomery limbs."""
 
-    def __init__(self, curve_id, num_instance, a, b, c, instance, witness):
+    def __init__(self, curve_id, num_instance, a, b, c, instance, witness, num_variables=None):
         self.curve_id = curve_id
         self.num_instance = num_instance          # formatted (includes the leading one), power of two
         self.a, self.b, self.c = a, b, c          # each: (row_ptr u64[n+1], col u64[nnz], coeff u64[nnz,4])
-        self.instance = instance                  # u64[num_instance, 4]
-        self.witness = witness                    # u64[num_witness, 4]
+        self.instance = instance                  # u64[num_instance, 4], or None (matrices only)
+        self.witness = witness                    # u64[num_witness, 4], or None (matrices only)
         self.num_constraints = len(a[0]) - 1
-        self.num_variables = num_instance + len(witness)
+        # without an assignment the variable count is given (Marlin.load_r1cs)
+        self.num_variables = num_instance + len(witness) if witness is not None else num_variables
+        self.circom = None                        # marlin_b200.circom.CircomInfo of an instance loaded from circom files
 
     def matrices(self):
         out = []
@@ -61,27 +63,40 @@ def _csr(rows_cols, rows_coeffs, n_rows):
     return row_ptr, col, coeff
 
 
+class Shape:
+    """The padded, squared shape of an instance with ni0 formatted inputs (One included), num_witness witnesses and
+    num_constraints rows [reference src/ahp/constraint_systems.rs:45-81, src/ahp/indexer.rs:151-167]:
+    ni = next_pow2(ni0) instance entries, the last `shift` = ni - ni0 of them zero; column c of a variable goes to c when
+    c < ni0 and to c + shift otherwise; with nv = ni + num_witness, `pad_rows` empty rows are appended when nv > nc, else
+    `pad_witness` witnesses equal to one; `size` = rows = variables of the result."""
+
+    def __init__(self, ni0, num_witness, num_constraints):
+        self.ni0 = ni0
+        self.ni = _next_pow2(ni0)
+        self.shift = self.ni - ni0
+        nv = self.ni + num_witness
+        self.pad_rows = max(nv - num_constraints, 0)
+        self.pad_witness = max(num_constraints - nv, 0)
+        self.size = max(nv, num_constraints)
+
+    def column(self, c):
+        return c if c < self.ni0 else c + self.shift
+
+
 def from_rows(curve_id, a_rows, b_rows, c_rows, instance, witness):
     """Generic (small) instance: *_rows[r] = [(coeff, col), ...] with canonical integer coefficients;
-    instance / witness are canonical integers (instance includes the leading one).  Pads and squares."""
+    instance / witness are canonical integers (instance includes the leading one).  Pads and squares (Shape)."""
     instance = list(instance)
     witness = list(witness)
-    ni = _next_pow2(len(instance))
-    shift = ni - len(instance)  # padding the instance moves every witness column up
-    old_ni = len(instance)
-    instance += [0] * shift
+    sh = Shape(len(instance), len(witness), len(a_rows))
+    ni = sh.ni
+    instance += [0] * sh.shift
 
     def remap(rows):
-        return [[(c, i if i < old_ni else i + shift) for c, i in row] for row in rows]
+        return [[(c, sh.column(i)) for c, i in row] for row in rows] + [[] for _ in range(sh.pad_rows)]
 
     a_rows, b_rows, c_rows = remap(a_rows), remap(b_rows), remap(c_rows)
-    nv = ni + len(witness)
-    nc = len(a_rows)
-    if nv > nc:
-        for rows in (a_rows, b_rows, c_rows):
-            rows += [[] for _ in range(nv - nc)]
-    else:
-        witness += [1] * (nc - nv)
+    witness += [1] * sh.pad_witness
     n = len(a_rows)
     mont = lambda v: fields.fr_to_mont(curve_id, v)
     mats = []
