@@ -23,6 +23,10 @@ pub struct b2m_vk {
     _p: [u8; 0],
 }
 #[repr(C)]
+pub struct b2m_pc_vk {
+    _p: [u8; 0],
+}
+#[repr(C)]
 pub struct b2m_matrix {
     pub row_ptr: *const u64,
     pub col: *const u64,
@@ -114,6 +118,17 @@ extern "C" {
                                     n_queries: usize, query_lc: *const usize, query_point: *const usize, n_points: usize,
                                     points: *const u64, opening_challenge: *const u64, out_w_xy: *mut u64, out_has_random_v: *mut c_int,
                                     out_random_v: *mut u64) -> c_int;
+    pub fn b2m_pc_vk_create(ctx: *mut b2m_ctx, curve: c_int, pc_variant: c_int, max_degree: usize, g_xy: *const u64, gamma_g_xy: *const u64,
+                            h_bytes: *const u8, beta_h_bytes: *const u8, n_bounds: usize, bounds: *const u64, bound_points: *const c_void,
+                            out: *mut *mut b2m_pc_vk) -> c_int;
+    pub fn b2m_pc_vk_destroy(vk: *mut b2m_pc_vk);
+    pub fn b2m_pc_check_combinations(vk: *mut b2m_pc_vk, n_sets: usize, comm_off: *const usize, comms: *const u8, comm_bounds: *const i64,
+                                     has_shifted: *const c_int, shifted: *const u8, lc_off: *const usize, lc_term_off: *const usize,
+                                     lc_comm: *const i64, lc_coeff: *const u64, point_off: *const usize, points: *const u64, w: *const u8,
+                                     has_random_v: *const c_int, random_v: *const u8, query_off: *const usize, query_lc: *const usize,
+                                     query_point: *const usize, evals: *const u8, challenges: *const u64, rng: *mut b2m_rng,
+                                     verdicts: *mut c_int) -> c_int;
+    pub fn b2m_pc_vk_timings(vk: *const b2m_pc_vk, json: *mut c_char, cap: usize) -> c_int;
     pub fn b2m_index_create(srs: *mut b2m_srs, pc_variant: c_int, num_constraints: usize, num_variables: usize,
                             num_instance_variables: usize, a: *const b2m_matrix, b: *const b2m_matrix, c: *const b2m_matrix,
                             out: *mut *mut b2m_index) -> c_int;

@@ -11,11 +11,15 @@
 //!   open_individual_opening_challenges        -> b2m_pc_open
 //!   open_combinations_individual_opening_...  -> b2m_ck_open_combinations
 //!
+//! The trait's single-set `check*` methods stay upstream: on the GPU one set costs one pairing-product latency (17-56 ms,
+//! DESIGN.md section 9).  Many sets at once go to the GPU through the inherent `check_combinations_many` (b2m_pc_check_combinations,
+//! DESIGN.md section 16); `batch_check` / `check` are its case with one LC per commitment.
+//!
 //! NOT compiled in this repository (no Rust toolchain in the build image).  Signatures follow ark-poly-commit 0.3.0 as recalled
 //! [U]; a maintainer should expect to touch lifetimes / bounds, not the marshalling, which is exercised through the ctypes twin of
 //! these calls (tests/test_prover_gpu.py::test_trim_and_open_combinations_level1, ::test_generic_rng_callback).
 use crate::{check, ffi, fr_mont_limbs, g1_from_limbs, g1_limbs, Context, Error as B2mError};
-use ark_bls12_381::{Bls12_381, Fr};
+use ark_bls12_381::{Bls12_381, Fr, G1Affine};
 use ark_ff::{BigInteger256, Field, One};
 use ark_poly::univariate::DensePolynomial;
 use ark_poly_commit::{
@@ -389,6 +393,167 @@ mod sonic_glue {
 
 b200_pc!(B200MarlinKZG10, UpMarlin, marlin_glue, false);
 b200_pc!(B200SonicKZG10, UpSonic, sonic_glue, true);
+
+// ---- batched check_combinations on the GPU ---------------------------------------------------------------------------------
+/// One `check_combinations` call's inputs, as the trait method takes them.
+pub struct OpeningSet<'a, C> {
+    pub lc_s: Vec<&'a LinearCombination<Fr>>,
+    pub commitments: Vec<&'a LabeledCommitment<C>>,
+    pub query_set: &'a QuerySet<Fr>,
+    pub evaluations: &'a Evaluations<Fr, Fr>,
+    pub proof: &'a [kzg10::Proof<Bls12_381>],
+    pub opening_challenge: Fr,
+}
+
+/// A device-side `PC::VerifierKey` (b2m_pc_vk): G2 points prepared once, reused by every batch.
+pub struct DeviceVerifierKey {
+    _ctx: Context,
+    vk: *mut ffi::b2m_pc_vk,
+}
+impl Drop for DeviceVerifierKey {
+    fn drop(&mut self) {
+        unsafe { ffi::b2m_pc_vk_destroy(self.vk) }
+    }
+}
+
+fn g2_uncompressed(p: &<Bls12_381 as ark_ec::PairingEngine>::G2Affine, out: &mut Vec<u8>) {
+    use ark_serialize::CanonicalSerialize;
+    p.serialize_uncompressed(&mut *out).expect("G2 serialization");
+}
+fn g1_compressed(p: &G1Affine, out: &mut Vec<u8>) {
+    use ark_serialize::CanonicalSerialize;
+    p.serialize(&mut *out).expect("G1 serialization");
+}
+fn fr_canonical(v: &Fr, out: &mut Vec<u8>) {
+    use ark_serialize::CanonicalSerialize;
+    v.serialize(&mut *out).expect("Fr serialization");
+}
+
+/// The arrays of b2m_pc_check_combinations for many sets: commitments, LCs and points in label order (upstream sorts all three).
+#[derive(Default)]
+struct SetArrays {
+    comm_off: Vec<usize>, comms: Vec<u8>, comm_bounds: Vec<i64>, has_shifted: Vec<c_int>, shifted: Vec<u8>,
+    lc_off: Vec<usize>, lc_term_off: Vec<usize>, lc_comm: Vec<i64>, lc_coeff: Vec<u64>,
+    point_off: Vec<usize>, points: Vec<u64>, w: Vec<u8>, has_rv: Vec<c_int>, rv: Vec<u8>,
+    query_off: Vec<usize>, q_lc: Vec<usize>, q_pt: Vec<usize>, evals: Vec<u8>, xi: Vec<u64>,
+}
+
+macro_rules! check_many {
+    ($name:ident, $comm:ty, $pc:expr, $split:expr) => {
+        impl $name {
+            /// `PC::VerifierKey` on the device: g, gamma g, h, beta h and the per-bound material of the upstream key.
+            pub fn device_verifier_key(ctx: Context, vk: &<Self as PolynomialCommitment<Fr, P>>::VerifierKey) -> Result<DeviceVerifierKey, B2mError> {
+                let (g, gamma_g, h, beta_h, max_degree, bounds, bound_points) = $split(vk);
+                let (mut gl, mut gg) = (Vec::new(), Vec::new());
+                g1_limbs(&g, &mut gl);
+                g1_limbs(&gamma_g, &mut gg);
+                let (mut hb, mut bhb) = (Vec::new(), Vec::new());
+                g2_uncompressed(&h, &mut hb);
+                g2_uncompressed(&beta_h, &mut bhb);
+                let mut out = std::ptr::null_mut();
+                check(unsafe {
+                    ffi::b2m_pc_vk_create(ctx.raw, ffi::B2M_CURVE_BLS12_381, $pc, max_degree, gl.as_ptr(), gg.as_ptr(), hb.as_ptr(), bhb.as_ptr(),
+                                          bounds.len(), bounds.as_ptr(), bound_points.as_ptr() as *const c_void, &mut out)
+                })?;
+                Ok(DeviceVerifierKey { _ctx: ctx, vk: out })
+            }
+
+            /// `check_combinations` of many independent sets in one GPU batch: Some(true) accepted, Some(false) rejected,
+            /// None malformed (an evaluation or random_v not below r cannot occur for ark types; a bounded MarlinKZG10
+            /// commitment without its shifted commitment can).  The randomisers come from `rng`.
+            pub fn check_combinations_many<R: RngCore>(vk: &DeviceVerifierKey, sets: &[OpeningSet<$comm>], rng: &mut R)
+                                                       -> Result<Vec<Option<bool>>, B2mError> {
+                let mut a = SetArrays { comm_off: vec![0], lc_off: vec![0], lc_term_off: vec![0], point_off: vec![0], query_off: vec![0], ..Default::default() };
+                for s in sets {
+                    let mut comms: Vec<&LabeledCommitment<$comm>> = s.commitments.clone();
+                    comms.sort_by(|x, y| x.label().cmp(y.label()));
+                    let ci: BTreeMap<&str, usize> = comms.iter().enumerate().map(|(i, c)| (c.label().as_str(), i)).collect();
+                    for c in &comms {
+                        let (comm, shifted) = $name::split_commitment(c.commitment());
+                        g1_compressed(&comm, &mut a.comms);
+                        a.comm_bounds.push(c.degree_bound().map(|d| d as i64).unwrap_or(-1));
+                        a.has_shifted.push(shifted.is_some() as c_int);
+                        g1_compressed(&shifted.unwrap_or_default(), &mut a.shifted);
+                    }
+                    a.comm_off.push(a.comm_bounds.len());
+                    let mut lcs = s.lc_s.clone();
+                    lcs.sort_by(|x, y| x.label().cmp(y.label()));
+                    for lc in &lcs {
+                        for (coeff, term) in lc.iter() {
+                            a.lc_comm.push(if term.is_one() { -1 } else { ci[term.try_into().expect("polynomial label")] as i64 });
+                            a.lc_coeff.extend_from_slice(&(coeff.0).0);
+                        }
+                        a.lc_term_off.push(a.lc_comm.len());
+                    }
+                    a.lc_off.push(a.lc_term_off.len() - 1);
+                    let li: BTreeMap<&str, usize> = lcs.iter().enumerate().map(|(i, lc)| (lc.label().as_str(), i)).collect();
+                    let mut point_of: BTreeMap<&str, Fr> = BTreeMap::new();
+                    for (_, (pl, p)) in s.query_set.iter() {
+                        point_of.insert(pl.as_str(), *p);
+                    }
+                    let pi: BTreeMap<&str, usize> = point_of.keys().enumerate().map(|(i, l)| (*l, i)).collect();
+                    for (p, proof) in point_of.values().zip(s.proof.iter()) {
+                        a.points.extend_from_slice(&(p.0).0);
+                        g1_compressed(&proof.w, &mut a.w);
+                        a.has_rv.push(proof.random_v.is_some() as c_int);
+                        fr_canonical(&proof.random_v.unwrap_or_default(), &mut a.rv);
+                    }
+                    a.point_off.push(a.has_rv.len());
+                    for (l, (pl, p)) in s.query_set.iter() {
+                        a.q_lc.push(li[l.as_str()]);
+                        a.q_pt.push(pi[pl.as_str()]);
+                        fr_canonical(&s.evaluations[&(l.clone(), *p)], &mut a.evals);
+                    }
+                    a.query_off.push(a.q_lc.len());
+                    a.xi.extend_from_slice(&(s.opening_challenge.0).0);
+                }
+                let mut verdicts = vec![0 as c_int; sets.len()];
+                let mut dynrng: &mut dyn RngCore = rng;
+                let mut desc = callback_rng(&mut dynrng);
+                check(unsafe {
+                    ffi::b2m_pc_check_combinations(vk.vk, sets.len(), a.comm_off.as_ptr(), a.comms.as_ptr(), a.comm_bounds.as_ptr(), a.has_shifted.as_ptr(),
+                                                   a.shifted.as_ptr(), a.lc_off.as_ptr(), a.lc_term_off.as_ptr(), a.lc_comm.as_ptr(), a.lc_coeff.as_ptr(),
+                                                   a.point_off.as_ptr(), a.points.as_ptr(), a.w.as_ptr(), a.has_rv.as_ptr(), a.rv.as_ptr(),
+                                                   a.query_off.as_ptr(), a.q_lc.as_ptr(), a.q_pt.as_ptr(), a.evals.as_ptr(), a.xi.as_ptr(), &mut desc,
+                                                   verdicts.as_mut_ptr())
+                })?;
+                Ok(verdicts.into_iter().map(|v| match v { 1 => Some(true), 0 => Some(false), _ => None }).collect())
+            }
+        }
+    };
+}
+
+impl B200MarlinKZG10 {
+    fn split_commitment(c: &marlin_pc::Commitment<Bls12_381>) -> (G1Affine, Option<G1Affine>) {
+        (c.comm.0, c.shifted_comm.map(|s| s.0))
+    }
+}
+impl B200SonicKZG10 {
+    fn split_commitment(c: &kzg10::Commitment<Bls12_381>) -> (G1Affine, Option<G1Affine>) {
+        (c.0, None)
+    }
+}
+type G2 = <Bls12_381 as ark_ec::PairingEngine>::G2Affine;
+fn marlin_vk_parts(vk: &marlin_pc::VerifierKey<Bls12_381>) -> (G1Affine, G1Affine, G2, G2, usize, Vec<u64>, Vec<u64>) {
+    let mut bounds = Vec::new();
+    let mut points = Vec::new();
+    for (d, p) in vk.degree_bounds_and_shift_powers.iter().flatten() {
+        bounds.push(*d as u64);
+        g1_limbs(p, &mut points);
+    }
+    (vk.vk.g, vk.vk.gamma_g, vk.vk.h, vk.vk.beta_h, vk.max_degree, bounds, points)
+}
+fn sonic_vk_parts(vk: &sonic_pc::VerifierKey<Bls12_381>) -> (G1Affine, G1Affine, G2, G2, usize, Vec<u64>, Vec<u8>) {
+    let mut bounds = Vec::new();
+    let mut points = Vec::new();
+    for (d, p) in vk.degree_bounds_and_neg_powers_of_h.iter().flatten() {
+        bounds.push(*d as u64);
+        g2_uncompressed(p, &mut points);
+    }
+    (vk.g, vk.gamma_g, vk.h, vk.beta_h, vk.max_degree, bounds, points)
+}
+check_many!(B200MarlinKZG10, marlin_pc::Commitment<Bls12_381>, ffi::B2M_PC_MARLIN_KZG10, marlin_vk_parts);
+check_many!(B200SonicKZG10, kzg10::Commitment<Bls12_381>, ffi::B2M_PC_SONIC_KZG10, sonic_vk_parts);
 
 /// `Marlin::<Fr, B200MarlinKZG10, FS>` -- the reference's own `index` / `prove` / `verify` with the GPU behind `PC`.
 pub type GpuMarlin<FS> = ark_marlin::Marlin<Fr, B200MarlinKZG10, FS>;

@@ -357,6 +357,57 @@ int b2m_ck_open_combinations(b2m_ck* ck, size_t n_polys, const uint64_t* const* 
                              const uint64_t* opening_challenge, uint64_t* out_w_xy, int* out_has_random_v,
                              uint64_t* out_random_v);
 
+/* `PC::VerifierKey` of MarlinKZG10 / SonicKZG10 [U ark-poly-commit 0.3 marlin_pc / sonic_pc VerifierKey], the key of
+ * b2m_pc_check_combinations, built from public data.  The key borrows the context, like b2m_vk.
+ *   max_degree           : the SRS max degree D (every bound must be <= D)
+ *   g_xy, gamma_g_xy     : powers_of_g[0] and powers_of_gamma_g[0] (affine x||y Montgomery)
+ *   h_bytes, beta_h_bytes: uncompressed G2 bytes, checked to be finite points of the twist (as b2m_vk_create checks them)
+ *   bounds[n_bounds]     : the enforced degree bounds (distinct)
+ *   bound_points         : per bound, MarlinKZG10: `degree_bounds_and_shift_powers`, the G1 point powers_of_g[D - bound] (x||y
+ *                          Montgomery limbs); SonicKZG10: `degree_bounds_and_neg_powers_of_h`, beta^-(D - bound) h (uncompressed G2)
+ * Errors: B2M_ERR_INVALID_ARG. */
+typedef struct b2m_pc_vk b2m_pc_vk;
+int b2m_pc_vk_create(b2m_ctx* ctx, int curve, int pc_variant, size_t max_degree, const uint64_t* g_xy, const uint64_t* gamma_g_xy,
+                     const uint8_t* h_bytes, const uint8_t* beta_h_bytes, size_t n_bounds, const uint64_t* bounds,
+                     const void* bound_points, b2m_pc_vk** out);
+void b2m_pc_vk_destroy(b2m_pc_vk* vk);
+
+/* `PC::check_combinations(vk, lc_s, commitments, query_set, evaluations, proof, opening_challenge, rng)` [U ark-poly-commit 0.3
+ * marlin_pc / sonic_pc check_combinations_individual_opening_challenges] for n_sets independent sets in one call.  `batch_check`
+ * is the case where every LC is one commitment with coefficient one, labelled as the commitment, and `check` is `batch_check` at
+ * one point: callers form those LCs themselves.  Set s owns consecutive ranges of the arrays below; every index inside a set
+ * (commitment, LC, point) is local to the set.  What the prover sends is ark-serialize bytes, what the verifier forms is
+ * Montgomery Fr limbs (4 u64):
+ *   commitments   : [comm_off[s], comm_off[s+1]): comms (compressed G1, sizeof(Fq) bytes each), comm_bounds (degree bound, -1 for
+ *                   None), and for MarlinKZG10 has_shifted / shifted (the compressed `shifted_comm`, read where has_shifted != 0 and
+ *                   the commitment is bounded; both may be NULL for SonicKZG10)
+ *   LCs           : [lc_off[s], lc_off[s+1]), in label order; LC l (a global index) has the terms [lc_term_off[l], lc_term_off[l+1]):
+ *                   lc_coeff[t] (Montgomery) times commitment lc_comm[t], or `LCTerm::One` when lc_comm[t] = -1
+ *   opening points: [point_off[s], point_off[s+1]), distinct, in point-label order: points (Montgomery), and the point's
+ *                   `kzg10::Proof` -- w (compressed G1), has_random_v, random_v (32 canonical little-endian bytes)
+ *   queries       : [query_off[s], query_off[s+1]): (query_lc, query_point) and the evaluation evals (32 canonical bytes)
+ *   challenges    : xi per set (Montgomery); challenge k is xi^k over the point's LCs in label order, MarlinKZG10 spending a
+ *                   second one on each degree-bounded LC
+ * verdicts[s] = 1 accepted, 0 rejected by the check, -1 malformed: a point that does not decode (b2m_g1_decode_ark's checks:
+ * flags, x < p, curve, BLS12-381 subgroup), an evaluation or random_v not below r, a bounded MarlinKZG10 commitment without
+ * has_shifted.  The points are decoded on the GPU; the checks of all sets are folded with one 128-bit randomiser per (set,
+ * point) from rng into a few MSMs and one pairing product on the GPU, and a failing batch is bisected with fresh randomisers
+ * as b2m_verify_batch does (DESIGN.md §16).  Upstream's `Err` cases fail the call with B2M_ERR_INVALID_ARG naming the set,
+ * before any work or rng draw: a bounded commitment in an LC of several terms (EquationHasDegreeBounds) or with a coefficient
+ * other than one, a degree bound the key does not enforce, an index out of its set's range, a repeated query, a point without
+ * a query.  rng == NULL fails with B2M_ERR_MISSING_RNG.  n_sets = 0 is allowed. */
+int b2m_pc_check_combinations(b2m_pc_vk* vk, size_t n_sets, const size_t* comm_off, const uint8_t* comms, const int64_t* comm_bounds,
+                              const int* has_shifted, const uint8_t* shifted, const size_t* lc_off, const size_t* lc_term_off,
+                              const int64_t* lc_comm, const uint64_t* lc_coeff, const size_t* point_off, const uint64_t* points,
+                              const uint8_t* w, const int* has_random_v, const uint8_t* random_v, const size_t* query_off,
+                              const size_t* query_lc, const size_t* query_point, const uint8_t* evals, const uint64_t* challenges,
+                              b2m_rng* rng, int* verdicts);
+/* Phase split of the last b2m_pc_check_combinations on this key, with b2m_verify_timings's keys where they apply: {"sets",
+ * "points", "decode_ms", "terms_ms" (the equations' bookkeeping, host threads), "g2_set_ms", "msm_tables_ms", "fold_ms" (the
+ * randomised scalar fold of every check, host), "msm_ms", "pairing_ms", "first_check_ms", "bisection_ms", "checks",
+ * "products", "total_ms"}. */
+int b2m_pc_vk_timings(const b2m_pc_vk* vk, char* json, size_t cap);
+
 /* ---- Level 2: prover ABI ---------------------------------------------------------------- */
 
 /* R1CS matrix in CSR form, as `ConstraintSystem::to_matrices()` yields it

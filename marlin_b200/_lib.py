@@ -113,6 +113,11 @@ def lib():
         L.b2m_ck_shift_power.argtypes = [vp, u64, vp]
         L.b2m_ck_commit.argtypes = [vp, sz, vp, vp, vp, vp, P(Rng), vp, vp, vp, vp, sz]
         L.b2m_ck_open_combinations.argtypes = [vp, sz, vp, vp, vp, vp, vp, vp, sz, sz, vp, vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, vp]
+        L.b2m_pc_vk_create.argtypes = [vp, ci, ci, sz, vp, vp, vp, vp, sz, vp, vp, P(vp)]
+        L.b2m_pc_vk_destroy.argtypes = [vp]
+        L.b2m_pc_vk_destroy.restype = None
+        L.b2m_pc_check_combinations.argtypes = [vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, P(Rng), vp]
+        L.b2m_pc_vk_timings.argtypes = [vp, ctypes.c_char_p, sz]
         if hasattr(L, "b2m_index_create"):
             L.b2m_index_create.argtypes = [vp, ci, sz, sz, sz, P(Matrix), P(Matrix), P(Matrix), P(vp)]
             L.b2m_r1cs_check.argtypes = [vp, ci, sz, sz, sz, P(Matrix), P(Matrix), P(Matrix), vp, vp, P(sz)]

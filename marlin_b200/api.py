@@ -350,6 +350,37 @@ class VerifierKey:
             self.handle = None
 
 
+class PcVerifierKey:
+    """`PC::VerifierKey` of MarlinKZG10 / SonicKZG10 (b2m_pc_vk), built by `Marlin.pc_verifier_key`."""
+
+    def __init__(self, ctx, handle, curve_id, pc, degree_bounds):
+        self.ctx, self.handle, self.curve_id, self.pc, self.degree_bounds = ctx, handle, curve_id, pc, degree_bounds
+
+    def timings(self):
+        """Phase split (ms) of the last check_combinations / batch_check: decode, terms, MSM tables, fold, MSMs, pairings."""
+        buf = ctypes.create_string_buffer(4096)
+        _lib.check(_lib.lib().b2m_pc_vk_timings(self.handle, buf, 4096))
+        return json.loads(buf.value.decode() or "{}")
+
+    def close(self):
+        if self.handle:
+            _lib.lib().b2m_pc_vk_destroy(self.handle)
+            self.handle = None
+
+
+class OpeningSet:
+    """The inputs of one `PC::check_combinations` (or `batch_check`) call.
+    commitments: {label: G1} with G1 compressed ark-serialize bytes or affine Montgomery limbs (`g1_to_bytes` converts);
+    shifted: {label: G1}, MarlinKZG10's `shifted_comm` of bounded commitments; degree_bounds: {label: bound} (absent = None);
+    lcs: [(label, [(coeff, commitment label or None for LCTerm::One)])] (None for `batch_check`: one LC per commitment);
+    query_set: [(lc label, (point label, point))]; evaluations: {(lc label, point): value}; proofs: [(w, random_v or None)],
+    one `kzg10::Proof` per point label in label order; challenge: the opening challenge xi.  Field elements are Python ints."""
+
+    def __init__(self, commitments, query_set, evaluations, proofs, challenge, lcs=None, degree_bounds=None, shifted=None):
+        self.commitments, self.query_set, self.evaluations, self.proofs = commitments, query_set, evaluations, proofs
+        self.challenge, self.lcs, self.degree_bounds, self.shifted = challenge, lcs, degree_bounds or {}, shifted or {}
+
+
 def _p2(n):
     s = 1
     while s < n:
@@ -474,6 +505,98 @@ def verify_many(entries, rng):
     kof = (ctypes.c_uint32 * max(n, 1))(*key_of)
     _lib.check(_lib.lib().b2m_verify_multi(len(keys), vks, n, kof, *args, ctypes.byref(rng.c) if rng is not None else None, verdicts))
     return [{1: True, 0: False}.get(verdicts[i]) for i in range(n)]
+
+
+def pc_check_arrays(cid, sets, identity, limbs_to_bytes):
+    """The arrays of b2m_pc_check_combinations (after n_sets, in argument order) for OpeningSets of curve cid: commitments
+    in label order, LCs in label order (identity: one per commitment, as `batch_check` forms them), points in point-label
+    order, the query set deduplicated.  limbs_to_bytes: affine limbs (k, 2 * Fq limbs) -> k compressed G1 points."""
+    r = fields.FR_MODULUS[cid]
+    fq_bytes = 8 * _lib.LIMBS[cid][1]
+    g1s, shifted = [], []
+    comm_off, bounds, has_shifted = [0], [], []
+    lc_off, term_off, lc_comm, coeffs = [0], [0], [], []
+    point_off, points, ws, has_rv, rvs = [0], [], [], [], []
+    query_off, q_lc, q_pt, evals, xis = [0], [], [], [], []
+    fr = lambda v: fields.fr_to_mont(cid, v % r)  # noqa: E731
+    canon = lambda v: int(v).to_bytes(32, "little")  # noqa: E731  (not reduced: a value >= r is the library's to reject)
+    for s in sets:
+        labels = sorted(s.commitments)
+        ci = {l: i for i, l in enumerate(labels)}
+        for l in labels:
+            g1s.append(s.commitments[l])
+            d = s.degree_bounds.get(l)
+            bounds.append(-1 if d is None else int(d))
+            sh = s.shifted.get(l)
+            has_shifted.append(0 if sh is None else 1)
+            shifted.append(bytes(fq_bytes) if sh is None else sh)
+        comm_off.append(len(g1s))
+        if identity:
+            if s.lcs is not None:
+                raise ValueError("batch_check takes no linear combinations")
+            lcs = [(l, [(1, l)]) for l in labels]
+        else:
+            lcs = sorted(s.lcs, key=lambda lc: lc[0])
+        li = {lc[0]: i for i, lc in enumerate(lcs)}
+        if len(li) != len(lcs):
+            raise ValueError("two linear combinations share a label")
+        for _, terms in lcs:
+            for c, t in terms:
+                if t is not None and t not in ci:
+                    raise ValueError(f"MissingPolynomial: no commitment labelled {t!r}")
+                lc_comm.append(-1 if t is None else ci[t])
+                coeffs.append(fr(c))
+            term_off.append(len(lc_comm))
+        lc_off.append(len(term_off) - 1)
+        queries = sorted(set((lc, (pl, int(pt))) for lc, (pl, pt) in s.query_set))
+        at = {}
+        for _, (pl, pt) in queries:
+            if at.setdefault(pl, pt) != pt:
+                raise ValueError(f"point label {pl!r} names two points")
+        pls = sorted(at)
+        pi = {pl: j for j, pl in enumerate(pls)}
+        if len(s.proofs) != len(pls):
+            raise ValueError(f"{len(s.proofs)} opening proofs for {len(pls)} points")
+        for pl, (w, rv) in zip(pls, s.proofs):
+            points.append(fr(at[pl]))
+            ws.append(w)
+            has_rv.append(0 if rv is None else 1)
+            rvs.append(canon(0 if rv is None else rv))
+        point_off.append(len(points))
+        for lc, (pl, pt) in queries:
+            if lc not in li:
+                raise ValueError(f"MissingLinearCombination: no LC labelled {lc!r}")
+            if (lc, pt) not in s.evaluations:
+                raise ValueError(f"MissingEvaluation for {lc!r} at point {pl!r}")
+            q_lc.append(li[lc])
+            q_pt.append(pi[pl])
+            evals.append(canon(s.evaluations[(lc, pt)]))
+        query_off.append(len(q_lc))
+        xis.append(fr(s.challenge))
+
+    def g1_blob(items):
+        out = np.zeros((max(len(items), 1), fq_bytes), dtype=np.uint8)
+        limbs = [i for i, it in enumerate(items) if not isinstance(it, (bytes, bytearray))]
+        for i, it in enumerate(items):
+            if isinstance(it, (bytes, bytearray)):
+                out[i] = np.frombuffer(bytes(it), dtype=np.uint8)
+        if limbs:
+            out[limbs] = limbs_to_bytes(np.stack([np.asarray(items[i], dtype=np.uint64).reshape(-1) for i in limbs])).reshape(-1, fq_bytes)
+        return out
+
+    def arr(vals, dtype):
+        return np.ascontiguousarray(np.asarray(vals if vals else [0], dtype=dtype))
+
+    def fr_arr(vals):
+        return np.ascontiguousarray(_lib.ints_to_limbs(vals or [0], 4))
+
+    def byte_arr(vals):
+        return np.frombuffer(b"".join(vals) or bytes(32), dtype=np.uint8).copy()
+
+    return [arr(comm_off, np.uint64), g1_blob(g1s), arr(bounds, np.int64), arr(has_shifted, np.int32), g1_blob(shifted),
+            arr(lc_off, np.uint64), arr(term_off, np.uint64), arr(lc_comm, np.int64), fr_arr(coeffs), arr(point_off, np.uint64),
+            fr_arr(points), g1_blob(ws), arr(has_rv, np.int32), byte_arr(rvs), arr(query_off, np.uint64), arr(q_lc, np.uint64),
+            arr(q_pt, np.uint64), byte_arr(evals), fr_arr(xis)]
 
 
 def max_degree(num_constraints, num_variables, num_non_zero):
@@ -1169,6 +1292,58 @@ class Marlin:
     def verify(self, vk, public_input, proof_bytes, rng):
         """`Marlin::verify` of one proof -> bool (malformed bytes are False)."""
         return self.verify_batch(vk, [public_input], [proof_bytes], rng)[0] is True
+
+    # -- PC::check_combinations (Level 1) --------------------------------------------------------------
+    def pc_verifier_key(self, srs, enforced_degree_bounds=()):
+        """`PC::VerifierKey` after `PC::trim`: g, gamma g, h, beta h and per enforced bound d MarlinKZG10's powers_of_g[D - d] or
+        SonicKZG10's beta^-(D - d) h, with the G2 half from the SRS's trapdoor or its source file (as `verifier_key`)."""
+        cid = self.curve_id
+        bounds = sorted(set(int(d) for d in enforced_degree_bounds))
+        D = srs.max_degree
+        h, beta_h, neg = g2_half(srs, bounds)
+        if self.pc == _lib.PC_MARLIN_KZG10:
+            powers = np.ascontiguousarray(srs.powers_limbs)
+            bound_points = np.ascontiguousarray(np.stack([powers[D - d] for d in bounds])) if bounds else None
+        else:
+            missing = [d for d in bounds if D - d not in neg]
+            if missing:
+                raise ValueError(f"the SRS holds no neg_powers_of_h for the degree bounds {missing}")
+            bound_points = np.frombuffer(b"".join(neg[D - d] for d in bounds), dtype=np.uint8).copy() if bounds else None
+        g = np.ascontiguousarray(srs.powers_limbs[0])
+        gamma_g = np.ascontiguousarray(srs.gamma_limbs[list(srs.gamma_indices).index(0)])
+        b = np.asarray(bounds, dtype=np.uint64)
+        handle = ctypes.c_void_p()
+        _lib.check(_lib.lib().b2m_pc_vk_create(self.ctx.handle, cid, self.pc, D, _lib.ptr(g), _lib.ptr(gamma_g),
+                                                _lib.ptr(np.frombuffer(h, dtype=np.uint8).copy()),
+                                                _lib.ptr(np.frombuffer(beta_h, dtype=np.uint8).copy()), len(b), _lib.ptr(b) if bounds else None,
+                                                _lib.ptr(bound_points), ctypes.byref(handle)))
+        return PcVerifierKey(self.ctx, handle, cid, self.pc, bounds)
+
+    def check_combinations(self, vk, sets, rng):
+        """`PC::check_combinations` for many independent OpeningSets in one GPU batch (b2m_pc_check_combinations).  rng: the
+        ZkRng / CallbackRng the batch randomisers are drawn from (unpredictable to the prover).  Returns True (accepted) / False
+        (rejected) / None (malformed: a point that does not decode, an evaluation or random_v not below r, a bounded MarlinKZG10
+        commitment without its shifted commitment) per set, as `verify_batch`."""
+        return self._pc_check(vk, sets, rng, identity=False)
+
+    def batch_check(self, vk, sets, rng):
+        """`PC::batch_check` for many OpeningSets: check_combinations with one LC per commitment, coefficient one, labelled as
+        the commitment (upstream orders both by label, so the challenges are the same).  Each set's `lcs` must be None."""
+        return self._pc_check(vk, sets, rng, identity=True)
+
+    def check(self, vk, opening_set, rng):
+        """`PC::check` of one OpeningSet at a single point: `batch_check` of that set -> True / False / None."""
+        if len({q[1][0] for q in opening_set.query_set}) != 1:
+            raise ValueError("check opens at a single point")
+        return self.batch_check(vk, [opening_set], rng)[0]
+
+    def _pc_check(self, vk, sets, rng, identity):
+        arrays = pc_check_arrays(vk.curve_id, sets, identity, lambda limbs: g1_to_bytes(self.ctx, vk.curve_id, limbs, True))
+        n = len(sets)
+        verdicts = np.zeros(max(n, 1), dtype=np.int32)
+        _lib.check(_lib.lib().b2m_pc_check_combinations(vk.handle, n, *[_lib.ptr(a) for a in arrays],
+                                                         ctypes.byref(rng.c) if rng is not None else None, _lib.ptr(verdicts)))
+        return [{1: True, 0: False}.get(int(verdicts[i])) for i in range(n)]
 
     def stage(self, index_pk, r1cs):
         """Copy (x, w) into HBM ahead of time (device-resident timing in bench.py)."""

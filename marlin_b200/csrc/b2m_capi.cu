@@ -920,6 +920,72 @@ int b2m_srs_check_powers(b2m_srs* srs, const uint8_t* h, const uint8_t* beta_h, 
   });
 }
 
+// ---- Level 1: PC verifier -------------------------------------------------------------------------
+struct b2m_pc_vk {
+  b2m_ctx* ctx;
+  int pc;
+  std::unique_ptr<PcVerifierBase> impl;
+};
+
+int b2m_pc_vk_create(b2m_ctx* ctx, int curve, int pc_variant, size_t max_degree, const uint64_t* g_xy, const uint64_t* gamma_g_xy,
+                     const uint8_t* h_bytes, const uint8_t* beta_h_bytes, size_t n_bounds, const uint64_t* bounds, const void* bound_points,
+                     b2m_pc_vk** out) {
+  return guard([&] {
+    B2M_REQUIRE(ctx && g_xy && gamma_g_xy && h_bytes && beta_h_bytes && out && (n_bounds == 0 || (bounds && bound_points)), B2M_ERR_INVALID_ARG,
+                "null argument");
+    require_curve(curve);
+    B2M_REQUIRE(pc_variant == B2M_PC_MARLIN_KZG10 || pc_variant == B2M_PC_SONIC_KZG10, B2M_ERR_INVALID_ARG, "unknown PC variant");
+    B2M_REQUIRE(ctx->cx.world <= 1, B2M_ERR_UNSUPPORTED, "verification on a multi-GPU context");
+    ctx->cx.use();
+    const PcVkArgs a{pc_variant, max_degree, g_xy, gamma_g_xy, h_bytes, beta_h_bytes, n_bounds, bounds, bound_points};
+    std::unique_ptr<b2m_pc_vk> vk(new b2m_pc_vk{ctx, pc_variant, nullptr});
+    const auto make = curve == B2M_CURVE_BLS12_381 ? make_pc_verifier_bls : curve == B2M_CURVE_BN254 ? make_pc_verifier_bn : make_pc_verifier_bls377;
+    vk->impl.reset(make(ctx->cx, a));
+    *out = vk.release();
+    ctx->children++;
+  });
+}
+
+void b2m_pc_vk_destroy(b2m_pc_vk* vk) {
+  if (!vk) return;
+  b2m_ctx* ctx = vk->ctx;
+  ctx->cx.use();
+  cudaStreamSynchronize(ctx->cx.stream);
+  delete vk;
+  if (--ctx->children == 0 && ctx->dead) b2m_release_ctx(ctx);
+}
+
+int b2m_pc_check_combinations(b2m_pc_vk* vk, size_t n_sets, const size_t* comm_off, const uint8_t* comms, const int64_t* comm_bounds,
+                              const int* has_shifted, const uint8_t* shifted, const size_t* lc_off, const size_t* lc_term_off,
+                              const int64_t* lc_comm, const uint64_t* lc_coeff, const size_t* point_off, const uint64_t* points,
+                              const uint8_t* w, const int* has_random_v, const uint8_t* random_v, const size_t* query_off,
+                              const size_t* query_lc, const size_t* query_point, const uint8_t* evals, const uint64_t* challenges,
+                              b2m_rng* rng, int* verdicts) {
+  return guard([&] {
+    B2M_REQUIRE(vk && (n_sets == 0 || (comm_off && lc_off && lc_term_off && point_off && query_off && challenges && verdicts)), B2M_ERR_INVALID_ARG,
+                "null argument");
+    const PcSets S{n_sets, comm_off, comms, comm_bounds, has_shifted, shifted, lc_off, lc_term_off, lc_comm, lc_coeff, point_off, points, w,
+                   has_random_v, random_v, query_off, query_lc, query_point, evals, challenges};
+    if (n_sets) {  // the arrays a non-empty range reads
+      const size_t nc = comm_off[n_sets] - comm_off[0], nt = lc_term_off[lc_off[n_sets]] - lc_term_off[lc_off[0]];
+      const size_t np = point_off[n_sets] - point_off[0], nq = query_off[n_sets] - query_off[0];
+      B2M_REQUIRE((nc == 0 || (comms && comm_bounds && (vk->pc == B2M_PC_SONIC_KZG10 || (has_shifted && shifted)))) && (nt == 0 || (lc_comm && lc_coeff)) &&
+                      (np == 0 || (points && w && has_random_v && random_v)) && (nq == 0 || (query_lc && query_point && evals)),
+                  B2M_ERR_INVALID_ARG, "null argument");
+    }
+    require_verify_rng(rng);
+    vk->ctx->cx.use();
+    vk->impl->check_combinations(S, rng, verdicts);
+  });
+}
+
+int b2m_pc_vk_timings(const b2m_pc_vk* vk, char* json, size_t cap) {
+  return guard([&] {
+    B2M_REQUIRE(vk && json && cap > 0, B2M_ERR_INVALID_ARG, "null argument");
+    snprintf(json, cap, "%s", vk->impl->timings_json.c_str());
+  });
+}
+
 int b2m_verify(b2m_vk* vk, const uint64_t* public_input, size_t n_input, const uint8_t* proof, size_t proof_len, b2m_rng* rng, int* ok) {
   int rc = guard([&] { B2M_REQUIRE(ok != nullptr, B2M_ERR_INVALID_ARG, "null argument"); });
   if (rc != B2M_OK) return rc;

@@ -4,6 +4,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "pc_check.hpp"
 
 struct b2m_srs;
 
@@ -38,6 +39,26 @@ struct VkArgs {
   const void* bound_points;
 };
 
+// `PC::VerifierKey` of MarlinKZG10 / SonicKZG10 (Level 1 of include/b2m.h: b2m_pc_vk_*, b2m_pc_check_combinations)
+struct PcVkArgs {
+  int pc;
+  size_t max_degree;
+  const uint64_t* g_xy;
+  const uint64_t* gamma_g_xy;
+  const uint8_t* h_bytes;
+  const uint8_t* beta_h_bytes;
+  size_t n_bounds;
+  const uint64_t* bounds;
+  const void* bound_points;
+};
+struct PcVerifierBase {
+  virtual ~PcVerifierBase() {}
+  // `PC::check_combinations` for S.n independent sets; verdicts[s] = 1 / 0 / -1 (malformed).  An `Err` of upstream's throws
+  // B2M_ERR_INVALID_ARG naming the set before any work or rng draw.
+  virtual void check_combinations(const PcSets& S, b2m_rng* rng, int* verdicts) = 0;
+  std::string timings_json;
+};
+
 // b2m_pairing_check for one curve (pairing_impl.cuh; instantiated with the verifier of that curve)
 template <class Fq>
 void pairing_check(Ctx& cx, size_t n_g2, const uint8_t* g2, size_t n_products, const size_t* off, const uint64_t* g1_xy, const uint32_t* g2_index,
@@ -51,5 +72,8 @@ void srs_check_powers(b2m_srs* srs, const uint8_t* h, const uint8_t* beta_h, siz
 VerifierBase* make_verifier_bls(Ctx& cx, const VkArgs& a);
 VerifierBase* make_verifier_bn(Ctx& cx, const VkArgs& a);
 VerifierBase* make_verifier_bls377(Ctx& cx, const VkArgs& a);
+PcVerifierBase* make_pc_verifier_bls(Ctx& cx, const PcVkArgs& a);
+PcVerifierBase* make_pc_verifier_bn(Ctx& cx, const PcVkArgs& a);
+PcVerifierBase* make_pc_verifier_bls377(Ctx& cx, const PcVkArgs& a);
 
 }  // namespace b2m

@@ -43,6 +43,64 @@ __global__ void g1_decode_kernel(const uint8_t* bytes, size_t n, Affine<Fq>* out
   st_words(out + i, p);
 }
 
+// The verifier half of a MarlinKZG10 / SonicKZG10 `VerifierKey`, as b2m_vk_create and b2m_pc_vk_create both take it: h and
+// beta h must be finite points of the twist; per degree bound, MarlinKZG10's shift power powers_of_g[D - d] (G1 limbs) is
+// appended to `shift`, SonicKZG10's beta^-(D - d) h (uncompressed G2) is checked like h.  g2_bytes receives h, beta h and the
+// SonicKZG10 points, g2set the same points prepared for the GPU pairing.
+template <class Fq>
+void pc_key_g2(Ctx& cx, int pc, const uint8_t* h_bytes, const uint8_t* beta_h_bytes, size_t n_bounds, const void* bound_points,
+               std::vector<Affine<Fq>>& shift, std::vector<uint8_t>& g2_bytes, std::unique_ptr<PairingG2Set<Fq>>& g2set) {
+  constexpr size_t G2_BYTES = 4 * Fq::N * 4;
+  G2Prepared<Fq> h, beta_h;
+  B2M_REQUIRE(g2_prepare<Fq>(h_bytes, &h) && g2_prepare<Fq>(beta_h_bytes, &beta_h), B2M_ERR_INVALID_ARG,
+              "h / beta_h is not a finite point of the G2 curve");
+  for (size_t k = 0; k < n_bounds; k++) {
+    if (pc == B2M_PC_MARLIN_KZG10) {
+      Affine<Fq> p;
+      memcpy(&p, static_cast<const uint64_t*>(bound_points) + k * 2 * (Fq::N / 2), sizeof(p));
+      shift.push_back(p);
+    } else {
+      G2Prepared<Fq> q;
+      B2M_REQUIRE(g2_prepare<Fq>(static_cast<const uint8_t*>(bound_points) + k * G2_BYTES, &q), B2M_ERR_INVALID_ARG,
+                  "neg_powers_of_h[%zu] is not a finite point of the G2 curve", k);
+    }
+  }
+  g2_bytes.assign(h_bytes, h_bytes + G2_BYTES);
+  g2_bytes.insert(g2_bytes.end(), beta_h_bytes, beta_h_bytes + G2_BYTES);
+  if (pc == B2M_PC_SONIC_KZG10)
+    g2_bytes.insert(g2_bytes.end(), static_cast<const uint8_t*>(bound_points), static_cast<const uint8_t*>(bound_points) + n_bounds * G2_BYTES);
+  g2set.reset(new PairingG2Set<Fq>(cx, g2_bytes.size() / G2_BYTES, g2_bytes.data()));
+}
+
+// Decode n compressed G1 points (FQ_BYTES each, back to back) on the GPU into dst (device); status (host) receives each point's
+// g1_decompress status and, when host_pts is given, the decoded points too
+template <class Fq>
+void decode_g1_bases(Ctx& cx, const std::vector<uint8_t>& bytes, size_t n, Affine<Fq>* dst, std::vector<int>& status, Affine<Fq>* host_pts) {
+  status.assign(n, 0);
+  if (!n) return;
+  DBuf<uint8_t> dbytes(cx, bytes.size());
+  DBuf<int> dstatus(cx, n);
+  dbytes.upload(bytes.data(), bytes.size());
+  g1_decode_kernel<Fq><<<div_up(n, 128), 128, 0, cx.stream>>>(dbytes.p, n, dst, dstatus.p);
+  B2M_CHECK_LAUNCH();
+  cx.launches++;
+  dstatus.download(status.data(), n);
+  if (host_pts) B2M_CUDA(cudaMemcpyAsync(host_pts, dst, n * sizeof(Affine<Fq>), cudaMemcpyDeviceToHost, cx.stream));
+  cx.sync();
+}
+
+// f(i) for i < n on the host's cores: for per-item work that is independent across items
+template <class F>
+void host_parallel(size_t n, F&& f) {
+  const unsigned nt = std::max(1u, std::min(std::thread::hardware_concurrency(), (unsigned)((n + 63) / 64)));
+  std::vector<std::thread> pool;
+  for (unsigned t = 0; t < nt; t++)
+    pool.emplace_back([&, t] {
+      for (size_t i = t; i < n; i += nt) f(i);
+    });
+  for (auto& th : pool) th.join();
+}
+
 template <class Fr, class Fq>
 struct MarlinVerifier : VerifierBase {
   using Pt = Affine<Fq>;
@@ -90,24 +148,7 @@ struct MarlinVerifier : VerifierBase {
     }
     B2M_REQUIRE(bidx_h < a.n_bounds && bidx_k < a.n_bounds, B2M_ERR_INVALID_ARG, "the key must carry the degree bounds |H| - 2 = %zu and |K| - 2 = %zu",
                 H - 2, K - 2);
-    G2Prepared<Fq> h, beta_h;
-    B2M_REQUIRE(g2_prepare<Fq>(a.h_bytes, &h) && g2_prepare<Fq>(a.beta_h_bytes, &beta_h), B2M_ERR_INVALID_ARG,
-                "h / beta_h is not a finite point of the G2 curve");
-    for (size_t k = 0; k < a.n_bounds; k++) {
-      if (pc == B2M_PC_MARLIN_KZG10) {
-        shared.push_back(pt_from_limbs(static_cast<const uint64_t*>(a.bound_points) + k * 2 * (Fq::N / 2)));
-      } else {
-        G2Prepared<Fq> q;
-        B2M_REQUIRE(g2_prepare<Fq>(static_cast<const uint8_t*>(a.bound_points) + k * 4 * FQ_BYTES, &q), B2M_ERR_INVALID_ARG,
-                    "neg_powers_of_h[%zu] is not a finite point of the G2 curve", k);
-      }
-    }
-    g2_bytes.assign(a.h_bytes, a.h_bytes + 4 * FQ_BYTES);
-    g2_bytes.insert(g2_bytes.end(), a.beta_h_bytes, a.beta_h_bytes + 4 * FQ_BYTES);
-    if (pc == B2M_PC_SONIC_KZG10)
-      g2_bytes.insert(g2_bytes.end(), static_cast<const uint8_t*>(a.bound_points),
-                      static_cast<const uint8_t*>(a.bound_points) + a.n_bounds * 4 * FQ_BYTES);
-    g2set.reset(new PairingG2Set<Fq>(cx, g2_points(), g2_bytes.data()));
+    pc_key_g2<Fq>(cx, pc, a.h_bytes, a.beta_h_bytes, a.n_bounds, a.bound_points, shared, g2_bytes, g2set);
     // IndexVerifierKey ToBytes [reference src/data_structures.rs:36-43]: index_info || index_comms
     put_u64(vk_bytes, nv);
     put_u64(vk_bytes, nc);
@@ -197,19 +238,9 @@ struct MarlinVerifier : VerifierBase {
   }
 
   // ---- 3. the verifier's transcript and check_combinations bookkeeping ---------------------------------------------
-  struct Term {
-    Fr c;
-    uint32_t base;
-  };
-  struct PointEq {  // plain + z W against h, W against beta h, bounded[k] against neg[k]
-    std::vector<Term> plain;
-    std::vector<std::pair<size_t, Term>> bounded;
-    Fr z;
-    uint32_t w;
-  };
-  struct ProofEq {
-    PointEq pt[2];
-  };
+  using Term = VerifyTerm<Fr>;
+  using PointEq = VerifyPoint<Fr>;
+  using ProofEq = VerifyEq<Fr>;  // two points: beta and gamma
 
   Fr sample_outside_h(FiatShamir& fs) const {
     for (;;) {
@@ -289,6 +320,7 @@ struct MarlinVerifier : VerifierBase {
     // check_combinations [U ark-poly-commit marlin_pc / sonic_pc]: per point, labels in BTreeSet order,
     // challenge xi^k, MarlinKZG10 spending a second challenge on each degree-bounded LC
     auto base = [&](int slot) { return base0 + (uint32_t)slot; };
+    E.pt.resize(2);
     for (int j = 0; j < 2; j++) {
       PointEq& pe = E.pt[j];
       Fr ch = one, combined = Fr::zero();
@@ -350,7 +382,7 @@ struct VerifyItems {
   std::vector<typename V::ProofEq> eqs;
   std::vector<uint32_t> key;         // per equation: its key
   std::vector<size_t> pt_lo, pt_hi;  // per equation: its proof's points [lo, hi) among the proof points
-  double ms_msm = 0, ms_pairing = 0, ms_first = 0;
+  double ms_fold = 0, ms_msm = 0, ms_pairing = 0, ms_first = 0;
   int checks = 0, products = 0;
 
   explicit VerifyItems(Ctx& c) : cx(c) {}
@@ -418,6 +450,7 @@ struct VerifyItems {
         }
         node_prod.push_back(prods.size());
       }
+      ms_fold += ms_since(t_level);
       Clock::time_point t0 = Clock::now();
       for (Fr& x : sc) x = x.to_canonical();
       const size_t nj = job_off.size();
@@ -506,19 +539,9 @@ struct VerifyItems {
     // 2. decode on the GPU, straight into the MSM base array behind the shared bases
     DBuf<Pt> bases(cx, S + n_pts);
     std::vector<Pt> host_pts(n_pts);
-    std::vector<int> status(n_pts);
+    std::vector<int> status;
     bases.upload(shared.data(), S);
-    if (n_pts) {
-      DBuf<uint8_t> dbytes(cx, bytes.size());
-      DBuf<int> dstatus(cx, n_pts);
-      dbytes.upload(bytes.data(), bytes.size());
-      g1_decode_kernel<Fq><<<div_up(n_pts, 128), 128, 0, cx.stream>>>(dbytes.p, n_pts, bases.p + S, dstatus.p);
-      B2M_CHECK_LAUNCH();
-      cx.launches++;
-      dstatus.download(status.data(), n_pts);
-      B2M_CUDA(cudaMemcpyAsync(host_pts.data(), bases.p + S, n_pts * sizeof(Pt), cudaMemcpyDeviceToHost, cx.stream));
-      cx.sync();
-    }
+    decode_g1_bases<Fq>(cx, bytes, n_pts, bases.p + S, status, host_pts.data());
     const double ms_decode = ms_since(t0);
     // 3. transcript and equations
     t0 = Clock::now();
@@ -530,19 +553,11 @@ struct VerifyItems {
       for (size_t k = 0; k < parsed[i].pt_off.size(); k++)
         if (status[p0 + k] != G1_OK) verdicts[i] = -1;
     }
-    {  // O(1) Fr work + O(|X|) per proof, independent across proofs: spread over the host's cores
-      const unsigned nt = std::max(1u, std::min(std::thread::hardware_concurrency(), (unsigned)((n + 63) / 64)));
-      std::vector<std::thread> pool;
-      for (unsigned t = 0; t < nt; t++)
-        pool.emplace_back([&, t] {
-          for (size_t i = t; i < n; i += nt)
-            if (verdicts[i] == 0) {
-              const uint32_t u = uniq[key_of[i]];
-              has_eq[i] = keys[u]->equations(parsed[i], host_pts.data() + (first[i] - S), first[i], sbase[u], inputs[i], n_inputs[i], all_eqs[i]);
-            }
-        });
-      for (auto& th : pool) th.join();
-    }
+    host_parallel(n, [&](size_t i) {  // O(1) Fr work + O(|X|) per proof
+      if (verdicts[i] != 0) return;
+      const uint32_t u = uniq[key_of[i]];
+      has_eq[i] = keys[u]->equations(parsed[i], host_pts.data() + (first[i] - S), first[i], sbase[u], inputs[i], n_inputs[i], all_eqs[i]);
+    });
     std::vector<size_t> proof_of;
     for (size_t i = 0; i < n; i++) {
       if (!has_eq[i]) continue;  // verdict -1 (malformed) or 0 (no shifted commitment for a bounded polynomial)
